@@ -12,11 +12,13 @@ same pre-roll (PREROLL untimed frames after initialisation so that the memory is
       e2e   : frames/s of `DiMPTracker.track(frame)` -- the public call: pinned HOST uint8 frame in, box out; the H2D copy of the
               frame and the D2H of the localisation result are inside the timed region (wall clock around the loop, max over ranks).
       roofline[]         : per-kernel CUDA-event timings inside this run (steepest-descent optimiser, backbone+head, apply_filter).
+      --dump-outputs DIR : after the timed steps, what the last device-timed step computed (box, peak score, score map, updated
+                           filter) as DIR/<name>.npy, so that two builds can be compared output for output on identical inputs.
       cpu_baseline       : the unmodified reference tracker (baseline/_ref) on rank 0's host cores, bounded sample.
       torch_cuda_baseline: the unmodified reference tracker on stock PyTorch-CUDA (cuDNN, TF32 off) on the same GPU -- what a
                            pytracking user runs today -- and the same reference tracker above the engine (`plugin.install()`).
   --impl reference
-      The UNMODIFIED reference `DiMP` tracker (baseline/_ref, staged from /root/reference by baseline/stage_reference.py), stock
+      The UNMODIFIED reference `DiMP` tracker (baseline/_ref, staged by baseline/stage_reference.py when available), stock
       PyTorch CPU path, timed as the reference times itself (time.time() around `tracker.track`,
       pytracking/evaluation/tracker.py:226-233).  One reference process per rank, host threads split evenly between the ranks,
       whole-job value = world * K / max-over-ranks time (gloo gather).
@@ -59,9 +61,8 @@ CONFIG = {"workload": "DiMP-50 single-GPU, synthetic 288x288 crops, 10 SD iters/
                 "the sample memory are the tracker's steady-state working set"}
 
 
-# dram__bytes_read.sum + dram__bytes_write.sum per launch from the committed `ncu --set full` captures of the same kernels at the same
-# sizes (profiles/r02x_ncu_summary_all_kernels.txt, profiles/r02x_ncu_summary_conv_tc.txt; tools/ncu_round.sh) -- not measured in this run
-NCU_TRAFFIC = {"sd_tc": 36251000 + 394000, "conv_chain": 149774000, "apply_filter": 726000}
+# NVIDIA H100 SXM data sheet (dense, 700 W): the denominators of the roofline fractions, not rates measured here
+H100_HBM_GBS, H100_BF16_TFLOPS = 3350.0, 989.0
 
 
 def parse():
@@ -72,12 +73,17 @@ def parse():
     ap.add_argument("--impl", default="b200", choices=["b200", "reference"])
     ap.add_argument("--precision", type=int, default=0)
     ap.add_argument("--no-baselines", action="store_true", help="skip cpu_baseline / torch_cuda_baseline (profiling runs)")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write what the last timed step computed to DIR/<name>.npy (native dimp50 arm only)")
     ap.add_argument("--config", default="dimp50", choices=["dimp50", "prdimp50", "atom", "tomp101", "eco", "dimp_simple"],
                     help="dimp50 = BASELINE configs[1] (the metric of record, native whole-frame tracker); the others time the UNMODIFIED "
                          "reference tracker of BASELINE configs[2] / [0] / [3] above the engine (plugin.install()) against the same tracker "
                          "on stock PyTorch-CUDA and PyTorch-CPU; eco / dimp_simple: the same for the reference ECO and SuperDiMPSimple trackers "
                          "(not BASELINE configurations; their optimiser seams were bound last)")
-    return ap.parse_args()
+    args = ap.parse_args()
+    if args.dump_outputs and (args.config != "dimp50" or args.impl != "b200"):
+        ap.error("--dump-outputs is implemented for the native dimp50 arm (--impl b200 --config dimp50)")
+    return args
 
 
 # ------------------------------------------------------------------------------------------------------------
@@ -85,9 +91,10 @@ def load_peaks():
     p = os.path.join(ROOT, "MEASURED_PEAKS.json")
     if os.path.exists(p):
         d = json.load(open(p))
-        return {"hbm_gbs": d.get("hbm_gbs", 6650.0), "bf16_tflops": d.get("bf16_tflops_sustained", d.get("bf16_tflops", 1590.0)),
-                "bf16_tflops_burst": d.get("bf16_tflops", 1590.0), "source": "measured (MEASURED_PEAKS.json)"}
-    return {"hbm_gbs": 6650.0, "bf16_tflops": 1590.0, "bf16_tflops_burst": 1590.0, "source": "fallback (B200_PROFILING.md)"}
+        return {"hbm_gbs": d.get("hbm_gbs", H100_HBM_GBS), "bf16_tflops": d.get("bf16_tflops_sustained", d.get("bf16_tflops", H100_BF16_TFLOPS)),
+                "bf16_tflops_burst": d.get("bf16_tflops", H100_BF16_TFLOPS), "source": "measured (MEASURED_PEAKS.json)"}
+    return {"hbm_gbs": H100_HBM_GBS, "bf16_tflops": H100_BF16_TFLOPS, "bf16_tflops_burst": H100_BF16_TFLOPS,
+            "source": "NVIDIA H100 SXM data sheet (not measured)"}
 
 
 class ClockSampler(threading.Thread):
@@ -130,6 +137,18 @@ class ClockSampler(threading.Thread):
                 continue
         return {"sm_mhz": float(np.median(sm)) if sm else None, "sm_max_mhz": mx or None, "reasons": sorted(reasons),
                 "samples": len(sm)}
+
+
+def device_info(index):
+    """The GPU a number was measured on and its power limit (part of every absolute number this script prints)."""
+    d = {"name": torch.cuda.get_device_name(index), "power_limit_w": None}
+    try:
+        r = subprocess.run(["nvidia-smi", "-i", str(index), "--query-gpu=power.limit", "--format=csv,noheader,nounits"],
+                           capture_output=True, text=True, timeout=30)
+        d["power_limit_w"] = float(r.stdout.strip())
+    except Exception:
+        pass
+    return d
 
 
 def host_cores():
@@ -301,6 +320,12 @@ def run_b200(args, rank, world, local_rank):
     torch.cuda.synchronize(); barrier()
     dev_ms = e0.elapsed_time(e1)
     launches = _lib.lib().b200trk_launch_count() - launches0
+    if args.dump_outputs:         # what the last timed step handed back (FrameInfo) and the state it computed, copied outside the timing
+        dump = {"target_bbox": np.array(list(trk.info.bbox), dtype=np.float64),
+                "max_score": np.array([trk.info.max_score], dtype=np.float64),
+                "flag": np.array([trk.info.flag], dtype=np.float64),
+                "scores": trk.engine.scores[0].float().cpu().numpy(),
+                "filter": trk.engine.filter.float().cpu().numpy()}
     f += W + K
     del dev_frames
 
@@ -364,35 +389,38 @@ def run_b200(args, rank, world, local_rank):
     roof = [
         {"kernel": ("sd_tc_kernel<18,0>" if sd_tc else "sd_kernel<18,4,0>") + " (DiMP steepest descent, n=50, 10 it, one launch)",
          "bound": "hbm", "achieved": sd_bytes / (sd_us * 1e-6) / 1e9, "peak": peaks["hbm_gbs"], "unit": "GB/s",
-         "frac": sd_bytes / (sd_us * 1e-6) / 1e9 / peaks["hbm_gbs"], "traffic": NCU_TRAFFIC["sd_tc"] if sd_tc else None, "us_per_launch": sd_us,
+         "frac": sd_bytes / (sd_us * 1e-6) / 1e9 / peaks["hbm_gbs"], "traffic": None, "us_per_launch": sd_us,
          "us_per_sd_iteration": sd_us / SD_ITERS, "algorithmic_bytes": sd_bytes,
          "fused_lower_bound": {"bytes": sd_once, "us_at_peak": sd_once / (peaks["hbm_gbs"] * 1e3), "frac": sd_once / (peaks["hbm_gbs"] * 1e3) / sd_us}},
-        {"kernel": "conv_tc_kernel chain (ResNet-50 -> layer3 + clf head, batch 1, 3xTF32 on tcgen05; whole forward)", "bound": "tensor",
+        {"kernel": "conv_tc_kernel chain (ResNet-50 -> layer3 + clf head, batch 1, 3xTF32 on wgmma; whole forward)", "bound": "tensor",
          "achieved": net_flops / (net_us * 1e-6) / 1e12, "peak": peaks["bf16_tflops"], "unit": "TFLOP/s",
-         "frac": net_flops / (net_us * 1e-6) / 1e12 / peaks["bf16_tflops"], "traffic": NCU_TRAFFIC["conv_chain"], "us_per_launch": net_us,
+         "frac": net_flops / (net_us * 1e-6) / 1e12 / peaks["bf16_tflops"], "traffic": None, "us_per_launch": net_us,
          "algorithmic_flops": net_flops, "mma_issue_flops": 3 * net_flops},
         {"kernel": "apply_filter_kernel<18,16> (classify, 1 sample)", "bound": "hbm", "achieved": af_bytes / (af_us * 1e-6) / 1e9,
-         "peak": peaks["hbm_gbs"], "unit": "GB/s", "frac": af_bytes / (af_us * 1e-6) / 1e9 / peaks["hbm_gbs"], "traffic": NCU_TRAFFIC["apply_filter"],
+         "peak": peaks["hbm_gbs"], "unit": "GB/s", "frac": af_bytes / (af_us * 1e-6) / 1e9 / peaks["hbm_gbs"], "traffic": None,
          "us_per_launch": af_us, "algorithmic_bytes": af_bytes},
     ]
     out = {
         "metric": METRIC, "value": world * K / (dev_ms * 1e-3), "unit": "frames/s", "n_gpus": world, "steps": K, "warmup": W,
         "ms_per_step": dev_ms / K, "higher_is_better": True, "scaling": "weak", "vs_baseline": None,
-        "dtype": "f32 (3xTF32 error-compensated tcgen05 convolutions and optimiser sweeps; fp32 CUDA-core correlation)" if args.precision == 0 else "f32",
+        "dtype": "f32 (3xTF32 error-compensated wgmma convolutions and optimiser sweeps; fp32 CUDA-core correlation)" if args.precision == 0 else "f32",
         "data": "synthetic", "config": CONFIG,
         "e2e": {"value": world * K / (host_ms * 1e-3), "unit": "frames/s", "h2d_bytes_per_step": H * Wd * 3 + 16 + MEMORY * 4,
                 "d2h_bytes_per_step": 64, "api": "pytracking_b200.tracker.DiMPTracker.track(uint8 frame) -> {'target_bbox'}",
                 "ms_per_frame_median": float(np.median(per_frame) * 1e3)},
         "gpu_launches": int(launches),
         "roofline": roof[0], "rooflines": roof, "peak_source": peaks["source"],
-        "traffic_source": "ncu --set full captures committed under profiles/r02x_ncu_summary_*.txt (same kernels, same sizes, separate run)",
         "tracking": {"mean_iou_vs_synthetic_ground_truth": float(np.mean(ious)), "sequences": len(ious), "frames_per_sequence": len(boxes),
                      "gather": "one all_gather of [frames,6] per sequence at the end (pytracking_b200/shard.py)"},
-        "clocks": clocks,
+        "clocks": clocks, "device": device_info(local_rank),
     }
     if not args.no_baselines and world == 1:            # the CPU / stock-CUDA baselines are N = 1 lines
         out["rooflines"] = roof + eco_rows(peaks)
         out.update(baselines(frames, bb, W))
+    if args.dump_outputs:
+        os.makedirs(args.dump_outputs, exist_ok=True)
+        for name, a in dump.items():
+            np.save(os.path.join(args.dump_outputs, name + ".npy"), a)
     print(json.dumps(out))
 
 

@@ -1,5 +1,5 @@
 /*
- * b200trk -- C ABI of the Blackwell (sm_100a) per-frame tracking engine.
+ * b200trk -- C ABI of the Hopper (sm_90a, H100) per-frame tracking engine.
  *
  * One shared library (pytracking_b200/libb200trk.so), plain C signatures: raw pointers, ints, floats.
  * No torch / ATen types cross this boundary.
@@ -43,10 +43,10 @@ int         b200trk_version(void);
 const char* b200trk_last_error(void);
 /* Debug aid: when B200TRK_SD_TRACE is set in the environment the SD optimiser kernels record 64 phase time stamps
  * (globaltimer ns) of CTA 0; this copies them to out_host[64]. */
-/* 1 when the most recent steepest-descent optimiser call ran the tcgen05 kernel (sd_tc.cu), 0 for the CUDA-core kernel */
+/* 1 when the most recent steepest-descent optimiser call ran the tensor-core kernel (sd_tc.cu), 0 for the CUDA-core kernel */
 int b200trk_sd_last_kernel(void);
 int b200trk_debug_sd_trace(unsigned long long* out_host);
-int b200trk_debug_sd_units(unsigned long long* out_host);   /* [16][16] per-unit pipeline stamps of the tcgen05 SD kernel */
+int b200trk_debug_sd_units(unsigned long long* out_host);   /* [16][16] per-unit pipeline stamps of the tensor-core SD kernel */
 /* Number of kernels this library has launched so far in this process (for bench.py's gpu_launches). */
 uint64_t    b200trk_launch_count(void);
 

@@ -1,7 +1,7 @@
 """TEST INFRASTRUCTURE ONLY -- records what the host half of the native whole-frame tracker (csrc/dimp_tracker.cu: plan_crop / commit)
 and its two small kernels (sample_patch, localize) must reproduce, from the UNMODIFIED reference DiMP tracker run on the CPU.
 
-    python -m oracle.gen_host_logic_golden          (needs the reference: baseline/_ref or /root/reference)
+    python -m oracle.gen_host_logic_golden [cfg2|stress|noaug|localize]      (needs a reference checkout: baseline/_ref or PYTRACKING_REFERENCE)
 
 Per configuration (`tests/golden/dimp_host_<name>.npz`): the scalar state after DiMP.initialize, and per frame the crop request
 (sample_patch's patch_coord), the score map, both dcf.max2d results and the flag of localize_advanced, the output box, the memory
@@ -10,6 +10,8 @@ update (slot, target box, learning rate, sample weights) and the optimiser itera
   stress  -- thresholds moved into the range random-init scores live in, so every branch of the decision tree
              (not_found / uncertain / hard_negative by either maximum / normal), memory wrap-around and train_skipping > 1 occur
   noaug   -- use_augmentation=False, filter_init_zero=True: the configuration the native initialisation implements
+and `tests/golden/dimp_localize_random.npz`: the reference's `DiMP.localize_target` (translation, scale index, flag) on the 400 seeded
+problems of tests/tracker_cases.py:random_localize_cases.
 """
 import os
 import sys
@@ -146,6 +148,35 @@ def record(name, cfg):
     np.savez_compressed(os.path.join(GOLDEN, "dimp_host_%s.npz" % name), **rec)
 
 
+def record_localize():
+    from oracle import ref_shims
+    ref_shims.install(prroi_cpu=False)
+    from pytracking.tracker.dimp.dimp import DiMP
+    from pytracking.utils import TrackerParams
+    sys.path.insert(0, os.path.join(ROOT, "tests"))
+    from tracker_cases import random_localize_cases
+    tv, scale_ind, flag = [], [], []
+    for trial, kw, scores, target_sz, sample_scales, sample_pos, pos in random_localize_cases():
+        trk = DiMP.__new__(DiMP)
+        p = TrackerParams()
+        for k, v in kw.items():
+            setattr(p, k, v)
+        p.target_neighborhood_scale = 2.2
+        trk.params = p
+        trk.output_window = None
+        trk.kernel_size = torch.Tensor([4, 4])
+        trk.img_support_sz = torch.Tensor([288, 288])
+        trk.target_sz = target_sz
+        trk.pos = pos
+        t, si, _, f = trk.localize_target(scores.clone().unsqueeze(1), sample_pos, sample_scales)
+        assert t.dtype == torch.float32
+        tv.append(t.numpy())
+        scale_ind.append(int(si))
+        flag.append(FLAG[f])
+    np.savez_compressed(os.path.join(GOLDEN, "dimp_localize_random.npz"), translation=np.array(tv, dtype=np.float32),
+                        scale_ind=np.array(scale_ind), flag=np.array(flag))
+
+
 if __name__ == "__main__":
-    for name in (sys.argv[1:] or list(CONFIGS)):
-        record(name, CONFIGS[name])
+    for name in (sys.argv[1:] or list(CONFIGS) + ["localize"]):
+        record_localize() if name == "localize" else record(name, CONFIGS[name])

@@ -1,4 +1,4 @@
-"""Builds pytracking_b200/libb200trk.so in-tree with nvcc for sm_100a (cross-compiles without a GPU)."""
+"""Builds pytracking_b200/libb200trk.so in-tree with nvcc for sm_90a (H100; cross-compiles without a GPU)."""
 import os
 import subprocess
 import sys
@@ -6,12 +6,13 @@ from concurrent.futures import ThreadPoolExecutor
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
-OBJ = os.path.join(HERE, "build")
+OBJ = os.path.join(HERE, "build", "sm_90a")      # objects of another target are never linked in
 LIB = os.path.join(HERE, "libb200trk.so")
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
-FLAGS = ["-gencode", "arch=compute_100a,code=sm_100a", "-lineinfo", "-O3", "-std=c++17",
-         "-Xcompiler", "-fPIC", "-Xcompiler", "-Wall", "-diag-suppress", "177",
-         "-Xcompiler", "-ffp-contract=off"]      # host float32 state arithmetic must not be fused (dimp_tracker.cu)
+ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]
+FLAGS = ARCH + ["-lineinfo", "-O3", "-std=c++17",
+                 "-Xcompiler", "-fPIC", "-Xcompiler", "-Wall", "-diag-suppress", "177",
+                 "-Xcompiler", "-ffp-contract=off"]      # host float32 state arithmetic must not be fused (dimp_tracker.cu)
 
 
 def _sources():
@@ -51,7 +52,7 @@ def build_library(force=False, verbose=False):
             list(ex.map(compile_one, jobs))
     objs = [os.path.join(OBJ, s[:-3] + ".o") for s in _sources()]
     if jobs or force or not os.path.exists(LIB):
-        cmd = [NVCC, "-shared", "-gencode", "arch=compute_100a,code=sm_100a", "-o", LIB] + objs
+        cmd = [NVCC, "-shared"] + ARCH + ["-o", LIB] + objs
         r = subprocess.run(cmd, capture_output=True, text=True)
         if r.returncode != 0:
             raise RuntimeError("link failed:\n%s\n%s" % (r.stdout, r.stderr))

@@ -71,7 +71,7 @@ extern "C" int b200trk_debug_sd_trace(unsigned long long* out_host) {
     return cudaMemcpy(out_host, p, 512, cudaMemcpyDeviceToHost) == cudaSuccess ? 0 : 1;
 }
 
-// debug: per-unit pipeline stamps of the tcgen05 SD kernel ([16 units][16] x u64 SM clocks, CTA 0, first adjoint sweep; cleared after the read)
+// debug: per-unit pipeline stamps of the tensor-core SD kernel ([16 units][16] x u64 SM clocks, CTA 0, first adjoint sweep; cleared after the read)
 extern "C" int b200trk_debug_sd_units(unsigned long long* out_host) {
     char* p = (char*)b200trk::workspace(4096, 3);
     if (!p || !out_host) return 1;

@@ -1,4 +1,4 @@
-// Shared host/device helpers for libb200trk (sm_100a only).
+// Shared host/device helpers for libb200trk (sm_90a only).
 #pragma once
 #ifndef B200_CPU_EMUL      // host builds of the *_kernels.cuh headers get these helpers restated by tests/cpu_emul/cuda_shim.h
 #include <cuda_runtime.h>

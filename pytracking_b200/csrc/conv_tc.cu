@@ -1,28 +1,26 @@
-// Stage 1 on the 5th-generation tensor cores: implicit-GEMM convolution (+ folded BN bias, residual add, ReLU) with
-// TMA-staged im2col tiles feeding tcgen05.mma, accumulators in TMEM.
+// Stage 1 on the Hopper tensor cores: implicit-GEMM convolution (+ folded BN bias, residual add, ReLU) with TMA-staged im2col
+// tiles feeding warpgroup MMAs (wgmma.mma_async), accumulators in registers.
 //
 //   D[m][n] = sum_k A[m][k] * W[n][k]     m = output pixel, n = output channel, k = (kh, kw, cin)
 //
 // fp32 fidelity on a TF32 datapath: every operand tile is split into a (hi, lo) pair of TF32-representable fp32 numbers,
-// x = hi + lo (+ <= 2^-22 |x|), and each K-step issues three MMAs A_lo*B_hi + A_hi*B_lo (into one fp32 TMEM accumulator) and
-// A_hi*B_hi (into another; summed in the epilogue) ("3xTF32"); the dropped A_lo*B_lo term is O(2^-22) relative. HBM/L2 only ever
-// hold (and move) plain fp32 activations and weights.
+// x = hi + lo (+ <= 2^-22 |x|), and each K step issues three MMAs: A_lo*B_hi + A_hi*B_lo into one fp32 accumulator and A_hi*B_hi
+// into another (summed in the epilogue) ("3xTF32"); the dropped A_lo*B_lo term is O(2^-22) relative. HBM/L2 only ever hold (and
+// move) plain fp32 activations and weights.
 //
-// Tiling: CTA = 128 output pixels (a BW x BH rectangle of one sample, rows ordered (y, x)) x BN output channels.
+// Tiling: CTA = 128 output pixels (a BW x BH rectangle of one sample, rows ordered (y, x)) x BN output channels (64 or 128).
 // K is walked in 128-byte blocks (32 input channels of one filter tap): one 4-D TMA box {32 ch, BW*stride, BH*stride, 1}
 // (element strides {1, stride, stride, 1}; halo / padding = TMA out-of-bounds zero fill) lands the A tile in the K-major
-// SWIZZLE_128B layout; a 2-D box {32, BN} does the same for the weights. Warp roles: warp 0 = TMA producer, warp 1 = TMEM allocator +
-// MMA issuer (both run their loops with the whole warp converged, elect.sync inside the instruction wrappers of tc_ptx.cuh),
-// warps 2-9 = operand converters during the main loop, then epilogue.
-// Operand conversion (default, a_tmem): the raw tile is the hi operand (the TF32 datapath truncates). A: converter thread = tile row,
-// hi | lo of its 16 elements straight into a 64-column TENSOR-MEMORY stage behind the accumulators (tcgen05.st), and the MMAs take A
-// from TMEM; B: lo = x - trunc(x) written next to the raw tile in shared memory (fence.proxy.async). The K loop was bound by
-// shared-memory bandwidth with both operands in shared memory (DESIGN.md sections 4.3 and 8).
-// Epilogue: tcgen05.ld -> registers -> smem transpose -> bias/residual/ReLU -> coalesced global stores; warps w and w+4 share a TMEM
-// lane quadrant and split the accumulator columns. Small layers use split-K over gridDim.z: the <= 8 split CTAs of a tile form a
-// thread-block cluster, stage their partial tiles in their own shared memory and each reduces its share of the tile through
-// distributed shared memory in split order (fixed order => bitwise deterministic); with more than 8 splits (or B200TRK_TC_CLUSTER=0)
-// the partial tiles go to an L2-resident workspace and a per-tile arrival counter releases the split CTAs.
+// SWIZZLE_128B layout; a 2-D box {32, BN} does the same for the weights. Warp roles: warps 0-7 = two consumer warpgroups (rows
+// 0-63 and 64-127 of the tile), warp 8 = TMA producer. A consumer k-block: wait for the stage, split the raw tiles in place
+// (hi over the raw value, lo into the neighbouring slot; element-wise, so the swizzle is irrelevant), make the writes visible to
+// the async proxy, meet the other warpgroup, issue 12 wgmmas (4 K steps x 3 products) and release the PREVIOUS stage once its
+// wgmma group has retired, so that the split of one k-block overlaps the MMAs of the one before.
+// Epilogue: registers -> shared-memory staging tile -> bias/residual/ReLU -> coalesced global stores. Small layers use split-K over
+// gridDim.z: the <= 8 split CTAs of a tile form a thread-block cluster, stage their partial tiles in their own shared memory and each
+// reduces its share of the tile through distributed shared memory in split order (fixed order => bitwise deterministic); with more
+// than 8 splits (or B200TRK_TC_CLUSTER=0) the partial tiles go to an L2-resident workspace and a per-tile arrival counter releases
+// the split CTAs.
 #include "net.cuh"
 #include "tc_ptx.cuh"
 #include <cuda.h>
@@ -31,33 +29,28 @@
 
 namespace b200trk {
 
-constexpr int TC_BM = 128;          // UMMA M
-constexpr int TC_KB = 32;           // fp32 elements per 128-byte K block
-constexpr int TC_THREADS = 192;     // 6 warps (CW = 4 converter/epilogue warps); CW = 8 -> 320 threads
+constexpr int TC_BM = 128;                  // tile rows: two warpgroups x 64 (wgmma M)
+constexpr int TC_KB = 32;                   // fp32 elements per 128-byte K block
+constexpr int TC_CT = 256;                  // consumer threads (warps 0-7)
+constexpr int TC_THREADS = TC_CT + 32;      // + the TMA producer warp
 constexpr int TC_MAX_STAGES = 6;
-constexpr int TC_EPI_PITCH = 36;    // floats per staged accumulator row (32 + 4: conflict-free 128-bit smem accesses)
+constexpr int TC_SMEM_MAX = 220 * 1024;
 
 struct TcParams {
     CUtensorMap a_map, b_map;       // raw fp32 activations (4-D) and weights (2-D)
     float* out_raw;
     const float* bias; const float* residual;
     float* ws; unsigned* counters;
-    unsigned long long* trace;     // optional [16 k-blocks][8] pipeline event stamps of CTA (0,0,0)
     unsigned long long* dbg;       // optional [ctas][8] phase time stamps (globaltimer ns); nullptr in production
     int BW, BH, tiles_w, tiles_h;
     int Hout, Wout, Cout, Cin;
     int ksz, stride, pad;
     int BN, stages;
     int total_kb, kb_per_split, splits, cblks;
-    int relu, split_mode;
+    int relu;
     int cluster_red; // 1: the split-K CTAs of a tile form a thread-block cluster (1,1,splits) and reduce their partial tiles through
                      //    distributed shared memory instead of an L2 workspace + arrival counter
     int prefetch_b;  // 1: the weight tiles of the first pipeline stages are requested before griddepcontrol.wait (they do not depend on the previous layer)
-    int acc2;        // 1: the two small products (A_lo*B_hi, A_hi*B_lo) accumulate in a TMEM accumulator of their own (columns BN..2BN)
-    int a_tmem;      // 1: the A operand goes through TENSOR memory: the converter warps (thread = tile row) write hi | lo of each k-block into a
-                     //    64-column TMEM stage behind the accumulators and the MMAs take A from there; shared memory then holds only the raw A
-                     //    tile and B_hi | B_lo (per k-block 80 KB of shared-memory traffic instead of 144 KB at BN = 64, DESIGN.md section 8)
-    int tmem_cols;   // TMEM allocation (power of two)
     uint32_t stage_bytes;
     uint32_t a_bytes, b_bytes;
 };
@@ -95,66 +88,59 @@ __device__ __forceinline__ float4 ld_dsmem_f4(uint32_t local_addr, uint32_t rank
     return v;
 }
 
-// CW = number of converter / epilogue warps (4 or 8). With 8, warps w and w+4 share a TMEM lane quadrant and split the
-// accumulator columns (32-column chunks) between them; the converter work per thread halves.
-template <int CW>
-__global__ void __launch_bounds__(64 + 32 * CW, 1) conv_tc_kernel(const __grid_constant__ TcParams P) {
-    constexpr int CT = 32 * CW;        // converter / epilogue threads
+template <int BN>
+__device__ __forceinline__ void tc_mma(float (&d)[BN / 2], uint64_t a, uint64_t b) {
+    if constexpr (BN == 64) wgmma_ss_n64(d, a, b);
+    else wgmma_ss_n128(d, a, b);
+}
+
+template <int BN>
+__global__ void __launch_bounds__(TC_THREADS, 1) conv_tc_kernel(const __grid_constant__ TcParams P) {
+    constexpr int NACC = BN / 2;                 // accumulator registers per thread and product group
+    constexpr uint32_t a_tile = (uint32_t)TC_BM * 128u;   // 16 KB slot regardless of the box size
+    constexpr uint32_t b_tile = (uint32_t)BN * 128u;
+    constexpr uint32_t b_off = 2u * a_tile;     // stage = A_hi | A_lo | B_hi | B_lo
+    constexpr int RP = BN + 4;                   // floats per staged accumulator row (conflict-free 128-bit accesses)
     extern __shared__ uint8_t tc_smem_raw[];
     __shared__ __align__(8) uint64_t s_full[TC_MAX_STAGES];
     __shared__ __align__(8) uint64_t s_empty[TC_MAX_STAGES];
-    __shared__ __align__(8) uint64_t s_ready[TC_MAX_STAGES];   // (hi, lo) split of the stage finished by the 4 converter warps
-    __shared__ __align__(8) uint64_t s_tmem_full;
-    __shared__ uint32_t s_tmem_base;
 
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    const uint32_t smem_base = (smem_u32(tc_smem_raw) + 1023u) & ~1023u;
-    const uint32_t a_tile = (uint32_t)TC_BM * 128u;                     // 16 KB slot regardless of the box size
-    const uint32_t b_tile = (uint32_t)P.BN * 128u;
+    uint8_t* sbase = tc_smem_raw + ((1024u - (smem_u32(tc_smem_raw) & 1023u)) & 1023u);
+    const uint32_t smem_base = smem_u32(sbase);
     const uint32_t stage_bytes = P.stage_bytes;
-    const uint32_t b_off = P.a_tmem ? a_tile : 2u * a_tile;            // B_hi | B_lo behind the A slot(s)
-    const uint32_t a_col0 = (uint32_t)(P.acc2 ? 2 * P.BN : P.BN);      // first TMEM column of the A stages (a_tmem)
+    float* red = reinterpret_cast<float*>(sbase);          // [128][RP] accumulator staging (the idle pipeline buffers)
 
     // tile coordinates
     const int tiles_per_sample = P.tiles_w * P.tiles_h;
     const int s = blockIdx.x / tiles_per_sample;
     const int trem = blockIdx.x - s * tiles_per_sample;
     const int th = trem / P.tiles_w, tw = trem - th * P.tiles_w;
-    const int n0 = blockIdx.y * P.BN;
+    const int n0 = blockIdx.y * BN;
     const int kb0 = blockIdx.z * P.kb_per_split;
     const int kb1 = min(P.total_kb, kb0 + P.kb_per_split);
     const int nkb = kb1 - kb0;
+    constexpr int nchunks = BN / 32;
     unsigned long long* dbg = P.dbg ? P.dbg + 8 * ((size_t)(blockIdx.z * gridDim.y + blockIdx.y) * gridDim.x + blockIdx.x) : nullptr;
     if (dbg && threadIdx.x == 0) dbg[0] = gtimer();                   // CTA start
-    unsigned long long* trace = (P.trace && blockIdx.x == 0 && blockIdx.y == 0 && blockIdx.z == 0) ? P.trace : nullptr;
 
     if (threadIdx.x == 0) {
-        for (int i = 0; i < P.stages; ++i) {
-            mbar_init(smem_u32(&s_full[i]), 1); mbar_init(smem_u32(&s_empty[i]), 1); mbar_init(smem_u32(&s_ready[i]), CW);
-        }
-        mbar_init(smem_u32(&s_tmem_full), 1);
+        for (int i = 0; i < P.stages; ++i) { mbar_init(smem_u32(&s_full[i]), 1); mbar_init(smem_u32(&s_empty[i]), TC_CT / 32); }
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     }
-    if (warp == 1) {
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(&s_tmem_base)), "r"((uint32_t)P.tmem_cols) : "memory");
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-    }
-    if (warp == 0 && lane == 0) {
+    if (warp == 8 && lane == 0) {
         asm volatile("prefetch.tensormap [%0];" ::"l"((uint64_t)&P.a_map) : "memory");
         asm volatile("prefetch.tensormap [%0];" ::"l"((uint64_t)&P.b_map) : "memory");
     }
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem_base = __shfl_sync(0xffffffffu, s_tmem_base, 0);     // provably warp-uniform (tc_ptx.cuh)
-    // Programmatic dependent launch: everything above (barrier init, TMEM allocation, descriptor prefetch) overlaps the
-    // tail of the previous layer's kernel; nothing below may touch global memory before the previous grid has completed.
+    // Programmatic dependent launch: everything above (barrier init, descriptor prefetch) overlaps the tail of the previous
+    // layer's kernel; nothing below may touch global memory before the previous grid has completed.
     if (dbg && threadIdx.x == 0) dbg[1] = gtimer();                   // prologue done
     asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
     // The weights are constants: the producer requests the B tiles of the first stages now, so that only the activation tiles
     // remain to be fetched once the previous layer has completed.
     int npre = 0;
-    if (warp == 0 && P.prefetch_b) {
+    if (warp == 8 && P.prefetch_b) {
         npre = min(P.stages, nkb);
         int tap = kb0 / P.cblks, cb = kb0 - tap * P.cblks;
         for (int it = 0; it < npre; ++it) {
@@ -167,360 +153,184 @@ __global__ void __launch_bounds__(64 + 32 * CW, 1) conv_tc_kernel(const __grid_c
     asm volatile("griddepcontrol.wait;" ::: "memory");
     if (dbg && threadIdx.x == 0) dbg[2] = gtimer();                   // previous grid complete
 
-    if (warp == 0) {
+    if (warp == 8) {
         // ===================== TMA producer (whole warp converged, elect.sync inside the wrappers: tc_ptx.cuh) ==========
-        {
-            const int x0 = tw * P.BW * P.stride - P.pad, y0 = th * P.BH * P.stride - P.pad;
-            int tap = kb0 / P.cblks, cb = kb0 - tap * P.cblks;
-            int kh = tap / P.ksz, kw = tap - kh * P.ksz;
-            int st = 0;
-            uint32_t ph = 0;
-            for (int it = 0; it < nkb; ++it) {
-                const uint32_t full = smem_u32(&s_full[st]);
-                if (it >= npre) {
-                    mbar_wait(smem_u32(&s_empty[st]), ph ^ 1u);
-                    mbar_expect_tx_elect(full, P.a_bytes + P.b_bytes);
-                }
-                if (trace && it < 16 && lane == 0) trace[it * 8 + 0] = gtimer();          // slot free
-                const uint32_t sa = smem_base + (uint32_t)st * stage_bytes;
-                tma_load_4d_elect(sa, &P.a_map, full, cb * TC_KB, x0 + kw, y0 + kh, s);                 // raw -> A_hi slot
-                if (it >= npre) tma_load_2d_elect(sa + b_off, &P.b_map, full, tap * P.Cin + cb * TC_KB, n0);   // raw -> B_hi slot
-                if (trace && it < 16 && lane == 0) trace[it * 8 + 1] = gtimer();          // loads issued
-                if (++cb == P.cblks) { cb = 0; ++tap; if (++kw == P.ksz) { kw = 0; ++kh; } }
-                if (++st == P.stages) { st = 0; ph ^= 1u; }
+        const int x0 = tw * P.BW * P.stride - P.pad, y0 = th * P.BH * P.stride - P.pad;
+        int tap = kb0 / P.cblks, cb = kb0 - tap * P.cblks;
+        int kh = tap / P.ksz, kw = tap - kh * P.ksz;
+        int st = 0;
+        uint32_t ph = 0;
+        for (int it = 0; it < nkb; ++it) {
+            const uint32_t full = smem_u32(&s_full[st]);
+            if (it >= npre) {
+                mbar_wait(smem_u32(&s_empty[st]), ph ^ 1u);
+                mbar_expect_tx_elect(full, P.a_bytes + P.b_bytes);
             }
-        }
-    } else if (warp == 1) {
-        // ===================== MMA issuer (whole warp converged, elect.sync inside the wrappers: tc_ptx.cuh) =====================
-        {
-            // instruction descriptor: D = F32, A = B = TF32, both K-major, N = BN, M = 128
-            const uint32_t idesc = (1u << 4) | (2u << 7) | (2u << 10) | ((uint32_t)(P.BN >> 3) << 17) | ((uint32_t)(TC_BM >> 4) << 24);
-            int st = 0;
-            uint32_t ph = 0;
-            for (int it = 0; it < nkb; ++it) {
-                mbar_wait(smem_u32(&s_ready[st]), ph);
-                tc_fence_after();
-                if (dbg && it == 0 && lane == 0) dbg[3] = gtimer();                // first operands landed and split
-                if (trace && it < 16 && lane == 0) trace[it * 8 + 4] = gtimer();          // MMA warp sees the stage
-                const uint32_t d_ah = make_smem_desc_lo(smem_base + (uint32_t)st * stage_bytes), d_al = d_ah + (a_tile >> 4);
-                const uint32_t d_bh = make_smem_desc_lo(smem_base + (uint32_t)st * stage_bytes + b_off), d_bl = d_bh + (b_tile >> 4);
-                const uint32_t a_tm = tmem_base + a_col0 + (uint32_t)st * 64u;      // hi columns 0..31, lo columns 32..63 (a_tmem)
-                // The fp32 accumulate of the tensor pipe truncates; its error grows with the number of dependent additions into
-                // one accumulator and with the accumulator's magnitude. The two correction products are ~2^-11 of the main one:
-                // in an accumulator of their own their rounding is negligible, and the main accumulator takes a third of the adds.
-                const uint32_t acc_lo = tmem_base + (P.acc2 ? (uint32_t)P.BN : 0u);
-                if (P.a_tmem) {
-#pragma unroll
-                    for (int k = 0; k < TC_KB / 8; ++k) {
-                        const uint32_t adv = (uint32_t)(k * 32 >> 4), kc = (uint32_t)(k * 8);
-                        const uint32_t first = (it > 0 || k > 0) ? 1u : 0u;
-                        tc_mma_tf32_ts_lo(acc_lo, a_tm + 32u + kc, d_bh + adv, idesc, first);
-                        tc_mma_tf32_ts_lo(acc_lo, a_tm + kc, d_bl + adv, idesc, 1u);
-                        tc_mma_tf32_ts_lo(tmem_base, a_tm + kc, d_bh + adv, idesc, P.acc2 ? first : 1u);
-                    }
-                } else {
-#pragma unroll
-                    for (int k = 0; k < TC_KB / 8; ++k) {
-                        const uint32_t adv = (uint32_t)(k * 32 >> 4);      // 8 tf32 = 32 bytes per UMMA K step
-                        const uint32_t first = (it > 0 || k > 0) ? 1u : 0u;
-                        tc_mma_tf32_lo(acc_lo, d_al + adv, d_bh + adv, idesc, first);
-                        tc_mma_tf32_lo(acc_lo, d_ah + adv, d_bl + adv, idesc, 1u);
-                        tc_mma_tf32_lo(tmem_base, d_ah + adv, d_bh + adv, idesc, P.acc2 ? first : 1u);
-                    }
-                }
-                tc_commit_elect(smem_u32(&s_empty[st]));
-                if (trace && it < 16 && lane == 0) trace[it * 8 + 5] = gtimer();          // MMAs + commit issued
-                if (++st == P.stages) { st = 0; ph ^= 1u; }
-            }
-            tc_commit_elect(smem_u32(&s_tmem_full));
+            const uint32_t sa = smem_base + (uint32_t)st * stage_bytes;
+            tma_load_4d_elect(sa, &P.a_map, full, cb * TC_KB, x0 + kw, y0 + kh, s);                    // raw -> A_hi slot
+            if (it >= npre) tma_load_2d_elect(sa + b_off, &P.b_map, full, tap * P.Cin + cb * TC_KB, n0);  // raw -> B_hi slot
+            if (++cb == P.cblks) { cb = 0; ++tap; if (++kw == P.ksz) { kw = 0; ++kh; } }
+            if (++st == P.stages) { st = 0; ph ^= 1u; }
         }
     } else {
-        // ===================== epilogue (warps 2..5) =====================
-        // TMEM -> registers (thread = accumulator row) -> per-warp smem transpose -> lanes own (row, 4 channels), so
-        // that every warp-level global access covers 4 rows x 128 contiguous bytes.
-        const int q = warp & 3;                          // TMEM lane quadrant this warp may access
-        const int ew = warp - 2;                         // 0..CW-1
-        const int chalf = ew >> 2;                       // which of the (CW / 4) column shares this warp takes
-        constexpr int CSH = CW / 4;
-        const int tile_lin = blockIdx.y * gridDim.x + blockIdx.x;
-        const int num_tiles = gridDim.x * gridDim.y;
-        const int nchunks = P.BN / 32;
-        const int lrow = lane >> 3, lcol = (lane & 7) * 4;
-        float* stg = reinterpret_cast<float*>(tc_smem_raw + (smem_base - smem_u32(tc_smem_raw))) + ew * (32 * TC_EPI_PITCH);
-        // ---- operand converter: raw fp32 tile (as landed by TMA) -> TF32 hi in place + TF32 lo in the neighbouring slot.
-        //      Element-wise and position-preserving, so the 128-byte swizzle is irrelevant here.
+        // ===================== consumer warpgroups: operand split + wgmma, then the accumulator staging =====================
+        const int ct = threadIdx.x, wg = ct >> 7;
+        float acc[NACC], acc2[NACC];                  // A_hi*B_hi | A_lo*B_hi + A_hi*B_lo
+#pragma unroll
+        for (int i = 0; i < NACC; ++i) { acc[i] = 0.f; acc2[i] = 0.f; }
+        constexpr int NA = (int)(a_tile / 16) / TC_CT, NB = (int)(b_tile / 16) / TC_CT;     // float4 per thread: 4 | 2 or 4
+        int st = 0, prev = 0;
+        uint32_t ph = 0;
+        for (int it = 0; it < nkb; ++it) {
+            mbar_wait(smem_u32(&s_full[st]), ph);
+            if (dbg && it == 0 && ct == 0) dbg[3] = gtimer();             // first operands landed
+            float4* a_hi = reinterpret_cast<float4*>(sbase + (size_t)st * stage_bytes);
+            float4* a_lo = a_hi + a_tile / 16;
+            float4* b_hi = reinterpret_cast<float4*>(sbase + (size_t)st * stage_bytes + b_off);
+            float4* b_lo = b_hi + b_tile / 16;
+            // all loads of the stage are issued before the first store (the compiler must not serialise them behind the stores)
+            float4 xa[NA], xb[NB];
+#pragma unroll
+            for (int j = 0; j < NA; ++j) xa[j] = a_hi[ct + TC_CT * j];
+#pragma unroll
+            for (int j = 0; j < NB; ++j) xb[j] = b_hi[ct + TC_CT * j];
+#pragma unroll
+            for (int j = 0; j < NA; ++j) { float4 h, l; split_tf32_4(xa[j], h, l); a_hi[ct + TC_CT * j] = h; a_lo[ct + TC_CT * j] = l; }
+#pragma unroll
+            for (int j = 0; j < NB; ++j) { float4 h, l; split_tf32_4(xb[j], h, l); b_hi[ct + TC_CT * j] = h; b_lo[ct + TC_CT * j] = l; }
+            asm volatile("fence.proxy.async.shared::cta;" ::: "memory");     // generic-proxy writes -> visible to wgmma
+            asm volatile("bar.sync 1, %0;" ::"n"(TC_CT) : "memory");          // both warpgroups read all of B
+            const uint32_t sa = smem_base + (uint32_t)st * stage_bytes + (uint32_t)wg * 64u * 128u;   // this warpgroup's 64 rows
+            const uint32_t sb = smem_base + (uint32_t)st * stage_bytes + b_off;
+            wgmma_fence();
+#pragma unroll
+            for (int k = 0; k < TC_KB / 8; ++k) {
+                const uint32_t adv = (uint32_t)k * 32u;                       // 8 tf32 = 32 bytes per K step
+                tc_mma<BN>(acc2, wg_desc(sa + a_tile + adv), wg_desc(sb + adv));
+                tc_mma<BN>(acc2, wg_desc(sa + adv), wg_desc(sb + b_tile + adv));
+                tc_mma<BN>(acc, wg_desc(sa + adv), wg_desc(sb + adv));
+            }
+            wgmma_commit();
+            wgmma_wait<1>();                       // the previous k-block's group has retired: its stage may be refilled
+            if (it > 0 && lane == 0) mbar_arrive(smem_u32(&s_empty[prev]));
+            prev = st;
+            if (++st == P.stages) { st = 0; ph ^= 1u; }
+        }
+        wgmma_wait<0>();
+        wg_reg_fence(acc); wg_reg_fence(acc2);
+        if (dbg && ct == 0) dbg[4] = gtimer();                            // accumulator complete
+        asm volatile("bar.sync 1, %0;" ::"n"(TC_CT) : "memory");              // every wgmma of both warpgroups has read its operands
         {
-            uint8_t* sbase = tc_smem_raw + (smem_base - smem_u32(tc_smem_raw));
-            const int et = threadIdx.x - 64;                       // 0..CT-1
-            constexpr int NA = 1024 / CT;                          // float4 of A per thread (8 or 4)
-            const int a_v4 = (int)(a_tile / 16), b_v4 = (int)(b_tile / 16);
-            for (int it = 0; it < nkb; ++it) {
-                const int st = it % P.stages;
-                const uint32_t ph = (uint32_t)(it / P.stages) & 1u;
-                mbar_wait(smem_u32(&s_full[st]), ph);
-                if (trace && it < 16 && et == 0) trace[it * 8 + 2] = gtimer();   // tile landed
-                float4* a_hi = reinterpret_cast<float4*>(sbase + (size_t)st * stage_bytes);
-                float4* a_lo = a_hi + a_v4;
-                float4* b_hi = reinterpret_cast<float4*>(sbase + (size_t)st * stage_bytes + b_off);
-                float4* b_lo = b_hi + b_v4;
-                const int nb = b_v4 / CT;                          // float4 of B per thread: BN * 8 / CT
-                if (P.a_tmem) {
-                    // A through tensor memory (CW = 8): thread = tile row q*32 + lane, warps w and w + 4 take the two 16-element halves of
-                    // the 32-element k-block; the 128-byte swizzle of the landed tile is undone in the address of each 16-byte chunk.
-                    const int row = q * 32 + lane;
-                    const uint8_t* arow = reinterpret_cast<const uint8_t*>(a_hi) + row * 128;
-                    float4 xr[4], xb[NA];
+            const int r0 = wg * 64 + ((ct & 127) >> 5) * 16 + (lane >> 2), c0 = 2 * (lane & 3);
 #pragma unroll
-                    for (int j = 0; j < 4; ++j) xr[j] = *reinterpret_cast<const float4*>(arow + (((chalf * 4 + j) ^ (row & 7)) << 4));
+            for (int j = 0; j < BN / 8; ++j)
 #pragma unroll
-                    for (int j = 0; j < NA; ++j) xb[j] = (j < nb) ? b_hi[et + CT * j] : make_float4(0.f, 0.f, 0.f, 0.f);
-                    uint32_t hi[16], lo[16];
-#pragma unroll
-                    for (int j = 0; j < 4; ++j) {
-                        const float4 l = tc_lo_trunc(xr[j]);
-                        hi[4 * j] = __float_as_uint(xr[j].x); hi[4 * j + 1] = __float_as_uint(xr[j].y); hi[4 * j + 2] = __float_as_uint(xr[j].z); hi[4 * j + 3] = __float_as_uint(xr[j].w);
-                        lo[4 * j] = __float_as_uint(l.x); lo[4 * j + 1] = __float_as_uint(l.y); lo[4 * j + 2] = __float_as_uint(l.z); lo[4 * j + 3] = __float_as_uint(l.w);
-                    }
-                    const uint32_t ta = tmem_base + ((uint32_t)(q * 32) << 16) + a_col0 + (uint32_t)st * 64u + (uint32_t)(chalf * 16);
-                    tmem_st16(ta, hi);
-                    tmem_st16(ta + 32u, lo);
-#pragma unroll
-                    for (int j = 0; j < NA; ++j) if (j < nb) b_lo[et + CT * j] = tc_lo_trunc(xb[j]);
-                    asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory");
-                    tc_fence_before();
-                } else {
-                // all loads of the stage are issued before the first store (the compiler must not serialise them
-                // behind the shared-memory stores): 8 float4 of A and up to 8 of B per thread
-                float4 xa[NA], xb[NA];
-#pragma unroll
-                for (int j = 0; j < NA; ++j) xa[j] = a_hi[et + CT * j];
-#pragma unroll
-                for (int j = 0; j < NA; ++j) xb[j] = (j < nb) ? b_hi[et + CT * j] : make_float4(0.f, 0.f, 0.f, 0.f);
-                if (P.split_mode == 2) {
-                    // the TF32 datapath ignores the 13 low mantissa bits of an fp32 operand, so the raw tile already IS the
-                    // hi operand (truncation split); only lo = x - trunc(x) (exact in fp32) has to be produced
-#pragma unroll
-                    for (int j = 0; j < NA; ++j) a_lo[et + CT * j] = tc_lo_trunc(xa[j]);
-#pragma unroll
-                    for (int j = 0; j < NA; ++j) if (j < nb) b_lo[et + CT * j] = tc_lo_trunc(xb[j]);
-                } else {
-                    // explicit round-to-nearest split (cvt.rna.tf32.f32 on both parts): the checker for mode 2
-#pragma unroll
-                    for (int j = 0; j < NA; ++j) {
-                        float4 h, l;
-                        split_tf32(xa[j].x, h.x, l.x); split_tf32(xa[j].y, h.y, l.y); split_tf32(xa[j].z, h.z, l.z); split_tf32(xa[j].w, h.w, l.w);
-                        a_hi[et + CT * j] = h; a_lo[et + CT * j] = l;
-                    }
-#pragma unroll
-                    for (int j = 0; j < NA; ++j) {
-                        if (j < nb) {
-                            float4 h, l;
-                            split_tf32(xb[j].x, h.x, l.x); split_tf32(xb[j].y, h.y, l.y); split_tf32(xb[j].z, h.z, l.z); split_tf32(xb[j].w, h.w, l.w);
-                            b_hi[et + CT * j] = h; b_lo[et + CT * j] = l;
-                        }
-                    }
-                }
-                }
-                asm volatile("fence.proxy.async.shared::cta;" ::: "memory");     // generic-proxy writes -> visible to tcgen05.mma
-                __syncwarp();
-                if (trace && it < 16 && et == 0) trace[it * 8 + 3] = gtimer();   // split done
-                if (lane == 0) asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(&s_ready[st])) : "memory");
-            }
+                for (int h = 0; h < 2; ++h)
+                    *reinterpret_cast<float2*>(red + (r0 + 8 * h) * RP + 8 * j + c0) =
+                        make_float2(acc[4 * j + 2 * h] + acc2[4 * j + 2 * h], acc[4 * j + 2 * h + 1] + acc2[4 * j + 2 * h + 1]);
         }
-        mbar_wait(smem_u32(&s_tmem_full), 0);
-        tc_fence_after();
-        if (dbg && threadIdx.x == 64) dbg[4] = gtimer();              // accumulator complete
-        if (P.splits == 1) {
-            // rows of this warp's quadrant handled by this lane: q*32 + i*4 + lrow
-            bool rvalid[8];
-            size_t roff[8];
-#pragma unroll
-            for (int i = 0; i < 8; ++i) {
-                const int row = q * 32 + i * 4 + lrow;
-                const int ly = row / P.BW, lx = row - ly * P.BW;
-                const int oy = th * P.BH + ly, ox = tw * P.BW + lx;
-                rvalid[i] = row < P.BW * P.BH && oy < P.Hout && ox < P.Wout;
-                roff[i] = (((size_t)s * P.Hout + oy) * P.Wout + ox) * P.Cout;
-            }
-            for (int c = chalf; c < nchunks; c += CSH) {
-                uint32_t v[32];
-                tmem_ld32(tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)(c * 32), v);
-                if (P.acc2) {
-                    uint32_t v2[32];
-                    tmem_ld32(tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)(P.BN + c * 32), v2);
-#pragma unroll
-                    for (int i = 0; i < 32; ++i) v[i] = __float_as_uint(__uint_as_float(v[i]) + __uint_as_float(v2[i]));
-                }
-                __syncwarp();
-#pragma unroll
-                for (int i = 0; i < 8; ++i)
-                    *reinterpret_cast<float4*>(stg + lane * TC_EPI_PITCH + 4 * i) =
-                        make_float4(__uint_as_float(v[4 * i]), __uint_as_float(v[4 * i + 1]), __uint_as_float(v[4 * i + 2]),
-                                    __uint_as_float(v[4 * i + 3]));
-                __syncwarp();
-                const int n = n0 + c * 32 + lcol;
-                const float4 bias = P.bias ? __ldg(reinterpret_cast<const float4*>(P.bias + n)) : make_float4(0.f, 0.f, 0.f, 0.f);
-                // all residual loads of the chunk are issued before the first dependent use (memory-level parallelism)
-                float4 res[8];
-                if (P.residual) {
-#pragma unroll
-                    for (int i = 0; i < 8; ++i)
-                        res[i] = rvalid[i] ? __ldg(reinterpret_cast<const float4*>(P.residual + roff[i] + n)) : make_float4(0.f, 0.f, 0.f, 0.f);
-                } else {
-#pragma unroll
-                    for (int i = 0; i < 8; ++i) res[i] = make_float4(0.f, 0.f, 0.f, 0.f);
-                }
-#pragma unroll
-                for (int i = 0; i < 8; ++i) {
-                    if (rvalid[i]) {
-                        float4 f = *reinterpret_cast<const float4*>(stg + (i * 4 + lrow) * TC_EPI_PITCH + lcol);
-                        tc_finish4(P, roff[i] + n, bias, res[i], f);
-                    }
-                }
-            }
-        } else if (P.cluster_red) {
-            // ---- split-K through distributed shared memory, phase A: this CTA's partial tile -> its own shared memory (the operand
-            //      pipeline buffers are idle: every MMA that read them has retired). Row pitch BN + 4 floats. ----
-            float* red = reinterpret_cast<float*>(tc_smem_raw + (smem_base - smem_u32(tc_smem_raw)));
-            const int RP = P.BN + 4;
-            for (int c = chalf; c < nchunks; c += CSH) {
-                uint32_t v[32];
-                tmem_ld32(tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)(c * 32), v);
-                if (P.acc2) {
-                    uint32_t v2[32];
-                    tmem_ld32(tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)(P.BN + c * 32), v2);
-#pragma unroll
-                    for (int i = 0; i < 32; ++i) v[i] = __float_as_uint(__uint_as_float(v[i]) + __uint_as_float(v2[i]));
-                }
-                float* dst = red + (size_t)(q * 32 + lane) * RP + c * 32;
-#pragma unroll
-                for (int i = 0; i < 8; ++i)
-                    *reinterpret_cast<float4*>(dst + 4 * i) = make_float4(__uint_as_float(v[4 * i]), __uint_as_float(v[4 * i + 1]),
-                                                                         __uint_as_float(v[4 * i + 2]), __uint_as_float(v[4 * i + 3]));
-            }
-        } else {
-            // ---- split-K: partial tile -> L2 workspace (coalesced), tile-wide arrival counter, then EVERY split CTA
-            //      reduces its share of the tile rows in split order (fixed order => deterministic) ----
-            float* wsp = P.ws + ((size_t)blockIdx.z * num_tiles + tile_lin) * TC_BM * P.BN;
-            for (int c = chalf; c < nchunks; c += CSH) {
-                uint32_t v[32];
-                tmem_ld32(tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)(c * 32), v);
-                if (P.acc2) {
-                    uint32_t v2[32];
-                    tmem_ld32(tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)(P.BN + c * 32), v2);
-#pragma unroll
-                    for (int i = 0; i < 32; ++i) v[i] = __float_as_uint(__uint_as_float(v[i]) + __uint_as_float(v2[i]));
-                }
-                __syncwarp();
-#pragma unroll
-                for (int i = 0; i < 8; ++i)
-                    *reinterpret_cast<float4*>(stg + lane * TC_EPI_PITCH + 4 * i) =
-                        make_float4(__uint_as_float(v[4 * i]), __uint_as_float(v[4 * i + 1]), __uint_as_float(v[4 * i + 2]),
-                                    __uint_as_float(v[4 * i + 3]));
-                __syncwarp();
-#pragma unroll
-                for (int i = 0; i < 8; ++i) {
-                    const int row = q * 32 + i * 4 + lrow;
-                    __stcg(reinterpret_cast<float4*>(wsp + (size_t)row * P.BN + c * 32 + lcol),
-                           *reinterpret_cast<const float4*>(stg + (i * 4 + lrow) * TC_EPI_PITCH + lcol));
-                }
-            }
-            __threadfence();
-            asm volatile("bar.sync 1, %0;" ::"n"(CT) : "memory");
-            if (threadIdx.x == 64) {
-                atomicAdd(&P.counters[2 * tile_lin], 1u);
-                long long t0 = clock64();
-                while (ld_acquire_u32(&P.counters[2 * tile_lin]) < (unsigned)P.splits)
-                    if (clock64() - t0 > TC_WAIT_LIMIT_CLOCKS) __trap();
-                __threadfence();
-                if (dbg) dbg[5] = gtimer();                           // all splits of the tile arrived
-            }
-            asm volatile("bar.sync 1, %0;" ::"n"(CT) : "memory");
-            // row groups (4 rows each, 32 per tile) are dealt round-robin to (split, warp)
-            for (int g = blockIdx.z + P.splits * ew; g < 32; g += P.splits * CW) {
-                const int row = g * 4 + lrow;
-                const int ly = row / P.BW, lx = row - ly * P.BW;
-                const int oy = th * P.BH + ly, ox = tw * P.BW + lx;
-                if (!(row < P.BW * P.BH && oy < P.Hout && ox < P.Wout)) continue;
-                const size_t obase = (((size_t)s * P.Hout + oy) * P.Wout + ox) * P.Cout;
-                for (int c = 0; c < nchunks; ++c) {
-                    const int n = n0 + c * 32 + lcol;
-                    const float* src = P.ws + ((size_t)tile_lin * TC_BM + row) * P.BN + c * 32 + lcol;
-                    const size_t zstride = (size_t)num_tiles * TC_BM * P.BN;
-                    const float4 bias = P.bias ? __ldg(reinterpret_cast<const float4*>(P.bias + n)) : make_float4(0.f, 0.f, 0.f, 0.f);
-                    const float4 res = P.residual ? __ldg(reinterpret_cast<const float4*>(P.residual + obase + n)) : make_float4(0.f, 0.f, 0.f, 0.f);
-                    float4 f = make_float4(0.f, 0.f, 0.f, 0.f);
-                    for (int z0 = 0; z0 < P.splits; z0 += 8) {     // 8 partial loads in flight, summed in split order
-                        float4 p[8];
-#pragma unroll
-                        for (int u = 0; u < 8; ++u)
-                            p[u] = (z0 + u < P.splits) ? __ldcg(reinterpret_cast<const float4*>(src + (size_t)(z0 + u) * zstride))
-                                                       : make_float4(0.f, 0.f, 0.f, 0.f);
-#pragma unroll
-                        for (int u = 0; u < 8; ++u) { f.x += p[u].x; f.y += p[u].y; f.z += p[u].z; f.w += p[u].w; }
-                    }
-                    tc_finish4(P, obase + n, bias, res, f);
-                }
-            }
-            asm volatile("bar.sync 1, %0;" ::"n"(CT) : "memory");
-            if (threadIdx.x == 64) {
-                // the last split CTA to finish its share re-arms both counters for the next launch
-                if (atomicAdd(&P.counters[2 * tile_lin + 1], 1u) == (unsigned)(P.splits - 1)) {
-                    P.counters[2 * tile_lin] = 0;
-                    P.counters[2 * tile_lin + 1] = 0;
-                    __threadfence();
-                }
-            }
-        }
-        tc_fence_before();
-        if (dbg && threadIdx.x == 64) dbg[6] = gtimer();              // epilogue done
     }
-    if (P.cluster_red && P.splits > 1) {
-        // ---- phase B: every thread of the cluster meets (all partial tiles are staged), then each split CTA sums its share of the
-        //      tile rows over the peers' shared memory in split order (fixed order => bitwise deterministic) and finishes them ----
-        cluster_sync_all();
-        if (dbg && threadIdx.x == 64) dbg[5] = gtimer();              // all splits of the tile staged
-        if (warp >= 2) {
-            const int ew = warp - 2, lrow = lane >> 3, lcol = (lane & 7) * 4;
-            const int RP = P.BN + 4, nchunks = P.BN / 32;
-            const uint32_t red_u32 = smem_base;
-            const int rank = (int)cluster_rank();
-            // work items of this CTA = (row group of 4 rows dealt round-robin to the splits) x (32-channel chunk), dealt round-robin to
-            // the warps: with 8 splits and BN = 64 every warp has exactly one item and all DSMEM / residual loads are in flight at once
-            const int my_groups = (32 - rank + P.splits - 1) / P.splits;
-            for (int item = ew; item < my_groups * nchunks; item += CW) {
+    __syncthreads();                              // the staged tile is complete
+
+    const int lrow = lane >> 3, lcol = (lane & 7) * 4;
+    if (P.splits == 1 || P.cluster_red) {
+        // each CTA finishes its share of the tile rows: row groups of 4 rows dealt round-robin to the split CTAs, summed over the
+        // peers' staged tiles in split order (fixed order => bitwise deterministic); work items = (row group, 32-channel chunk)
+        if (P.cluster_red) cluster_sync_all();
+        if (dbg && threadIdx.x == 0) dbg[5] = gtimer();                   // all splits of the tile staged
+        if (warp < 8) {
+            const int rank = P.cluster_red ? (int)cluster_rank() : 0;
+            const int nsplit = P.cluster_red ? P.splits : 1;
+            const int my_groups = (32 - rank + nsplit - 1) / nsplit;
+            for (int item = warp; item < my_groups * nchunks; item += TC_CT / 32) {
                 const int gi = item / nchunks, c = item - gi * nchunks;
-                const int g = rank + P.splits * gi;
-                const int row = g * 4 + lrow;
+                const int row = (rank + nsplit * gi) * 4 + lrow;
                 const int ly = row / P.BW, lx = row - ly * P.BW;
                 const int oy = th * P.BH + ly, ox = tw * P.BW + lx;
                 if (!(row < P.BW * P.BH && oy < P.Hout && ox < P.Wout)) continue;
                 const size_t obase = (((size_t)s * P.Hout + oy) * P.Wout + ox) * P.Cout;
                 const int n = n0 + c * 32 + lcol;
-                const uint32_t a = red_u32 + (uint32_t)((row * RP + c * 32 + lcol) * 4);
                 const float4 bias = P.bias ? __ldg(reinterpret_cast<const float4*>(P.bias + n)) : make_float4(0.f, 0.f, 0.f, 0.f);
                 const float4 res = P.residual ? __ldg(reinterpret_cast<const float4*>(P.residual + obase + n)) : make_float4(0.f, 0.f, 0.f, 0.f);
-                float4 pv[8];
+                float4 f;
+                if (!P.cluster_red) {
+                    f = *reinterpret_cast<const float4*>(red + row * RP + c * 32 + lcol);
+                } else {
+                    const uint32_t a = smem_base + (uint32_t)((row * RP + c * 32 + lcol) * 4);
+                    float4 pv[8];
 #pragma unroll
-                for (int u = 0; u < 8; ++u) pv[u] = (u < P.splits) ? ld_dsmem_f4(a, (uint32_t)u) : make_float4(0.f, 0.f, 0.f, 0.f);
-                float4 f = make_float4(0.f, 0.f, 0.f, 0.f);
+                    for (int u = 0; u < 8; ++u) pv[u] = (u < P.splits) ? ld_dsmem_f4(a, (uint32_t)u) : make_float4(0.f, 0.f, 0.f, 0.f);
+                    f = make_float4(0.f, 0.f, 0.f, 0.f);
 #pragma unroll
-                for (int u = 0; u < 8; ++u) { f.x += pv[u].x; f.y += pv[u].y; f.z += pv[u].z; f.w += pv[u].w; }
+                    for (int u = 0; u < 8; ++u) { f.x += pv[u].x; f.y += pv[u].y; f.z += pv[u].z; f.w += pv[u].w; }
+                }
                 tc_finish4(P, obase + n, bias, res, f);
             }
         }
-        // No CTA may leave (and release its shared memory) while a peer still reads it.  The peers' values are in registers (consumed by
-        // the sums above) before a thread arrives, and nothing written here is read through the barrier, so the arrival carries no
-        // memory ordering: a releasing arrival would wait for the global stores of the finished rows to drain (~0.5 us per layer).
-        asm volatile("barrier.cluster.arrive.relaxed.aligned;" ::: "memory");
-        asm volatile("barrier.cluster.wait.aligned;" ::: "memory");
-        if (dbg && threadIdx.x == 64) dbg[6] = gtimer();
+        if (P.cluster_red) {
+            // No CTA may leave (and release its shared memory) while a peer still reads it. The peers' values are in registers
+            // (consumed by the sums above) before a thread arrives, so the arrival carries no memory ordering.
+            asm volatile("barrier.cluster.arrive.relaxed.aligned;" ::: "memory");
+            asm volatile("barrier.cluster.wait.aligned;" ::: "memory");
+        }
+    } else if (warp < 8) {
+        // ---- split-K: partial tile -> L2 workspace (coalesced), tile-wide arrival counter, then EVERY split CTA
+        //      reduces its share of the tile rows in split order (fixed order => deterministic) ----
+        const int tile_lin = blockIdx.y * gridDim.x + blockIdx.x;
+        const int num_tiles = gridDim.x * gridDim.y;
+        float* wsp = P.ws + ((size_t)blockIdx.z * num_tiles + tile_lin) * TC_BM * BN;
+        for (int i = threadIdx.x; i < TC_BM * BN / 4; i += TC_CT) {
+            const int row = i / (BN / 4), c4 = i - row * (BN / 4);
+            __stcg(reinterpret_cast<float4*>(wsp + (size_t)row * BN + 4 * c4), *reinterpret_cast<const float4*>(red + row * RP + 4 * c4));
+        }
+        __threadfence();
+        asm volatile("bar.sync 1, %0;" ::"n"(TC_CT) : "memory");
+        if (threadIdx.x == 0) {
+            atomicAdd(&P.counters[2 * tile_lin], 1u);
+            long long t0 = clock64();
+            while (ld_acquire_u32(&P.counters[2 * tile_lin]) < (unsigned)P.splits)
+                if (clock64() - t0 > TC_WAIT_LIMIT_CLOCKS) __trap();
+            __threadfence();
+            if (dbg) dbg[5] = gtimer();                               // all splits of the tile arrived
+        }
+        asm volatile("bar.sync 1, %0;" ::"n"(TC_CT) : "memory");
+        // row groups (4 rows each, 32 per tile) are dealt round-robin to (split, warp)
+        for (int g = blockIdx.z + P.splits * warp; g < 32; g += P.splits * (TC_CT / 32)) {
+            const int row = g * 4 + lrow;
+            const int ly = row / P.BW, lx = row - ly * P.BW;
+            const int oy = th * P.BH + ly, ox = tw * P.BW + lx;
+            if (!(row < P.BW * P.BH && oy < P.Hout && ox < P.Wout)) continue;
+            const size_t obase = (((size_t)s * P.Hout + oy) * P.Wout + ox) * P.Cout;
+            for (int c = 0; c < nchunks; ++c) {
+                const int n = n0 + c * 32 + lcol;
+                const float* src = P.ws + ((size_t)tile_lin * TC_BM + row) * BN + c * 32 + lcol;
+                const size_t zstride = (size_t)num_tiles * TC_BM * BN;
+                const float4 bias = P.bias ? __ldg(reinterpret_cast<const float4*>(P.bias + n)) : make_float4(0.f, 0.f, 0.f, 0.f);
+                const float4 res = P.residual ? __ldg(reinterpret_cast<const float4*>(P.residual + obase + n)) : make_float4(0.f, 0.f, 0.f, 0.f);
+                float4 f = make_float4(0.f, 0.f, 0.f, 0.f);
+                for (int z0 = 0; z0 < P.splits; z0 += 8) {     // 8 partial loads in flight, summed in split order
+                    float4 p[8];
+#pragma unroll
+                    for (int u = 0; u < 8; ++u)
+                        p[u] = (z0 + u < P.splits) ? __ldcg(reinterpret_cast<const float4*>(src + (size_t)(z0 + u) * zstride))
+                                                   : make_float4(0.f, 0.f, 0.f, 0.f);
+#pragma unroll
+                    for (int u = 0; u < 8; ++u) { f.x += p[u].x; f.y += p[u].y; f.z += p[u].z; f.w += p[u].w; }
+                }
+                tc_finish4(P, obase + n, bias, res, f);
+            }
+        }
+        asm volatile("bar.sync 1, %0;" ::"n"(TC_CT) : "memory");
+        if (threadIdx.x == 0) {
+            // the last split CTA to finish its share re-arms both counters for the next launch
+            if (atomicAdd(&P.counters[2 * tile_lin + 1], 1u) == (unsigned)(P.splits - 1)) {
+                P.counters[2 * tile_lin] = 0;
+                P.counters[2 * tile_lin + 1] = 0;
+                __threadfence();
+            }
+        }
     }
-    __syncthreads();
-    if (warp == 1) {
-        tc_fence_after();
-        asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"((uint32_t)P.tmem_cols) : "memory");
-    }
+    if (dbg && threadIdx.x == 0) dbg[6] = gtimer();                       // epilogue done
 }
 
 // ------------------------------------------------------------------------------------------------------------
@@ -663,23 +473,17 @@ static int tc_configure(b200trk_net* net, const Op& op, TcConv* tc, int S) {
     if (op.Cout % BN != 0 || (BN != 64 && BN != 128)) BN = 64;
     P.BN = BN;
     P.b_bytes = (uint32_t)BN * 128u;
-    P.acc2 = env_int("B200TRK_TC_ACC2", 1);
-    P.split_mode = env_int("B200TRK_TC_SPLIT_MODE", 2);
-    P.a_tmem = (env_int("B200TRK_TC_ATMEM", 1) && env_int("B200TRK_TC_CW", 8) != 4 && P.split_mode == 2) ? 1 : 0;
-    const uint32_t stage_bytes = (P.a_tmem ? 1u : 2u) * TC_BM * 128u + 2u * P.b_bytes;
+    const uint32_t stage_bytes = 2u * TC_BM * 128u + 2u * P.b_bytes;     // A_hi | A_lo | B_hi | B_lo
     P.stage_bytes = stage_bytes;
-    const int occ = env_int("B200TRK_TC_OCC", 1);                 // CTAs per SM the shared-memory footprint is sized for
-    int stages = (int)(((occ >= 2 ? 98u : 200u) * 1024u) / stage_bytes);
+    int stages = (int)((TC_SMEM_MAX - 1024u) / stage_bytes);
     if (stages > TC_MAX_STAGES) stages = TC_MAX_STAGES;
-    const int acc_cols = P.acc2 ? 2 * BN : BN;
-    if (P.a_tmem && stages > (512 - acc_cols) / 64) stages = (512 - acc_cols) / 64;      // one 64-column TMEM stage per shared-memory stage
+    if (stages > P.total_kb) stages = P.total_kb;
     if (stages < 2) stages = 2;
-    if (stages > P.total_kb) stages = P.total_kb < 2 ? 2 : P.total_kb;
     P.stages = stages;
     const int ctas = m_tiles * (op.Cout / BN);
     int splits = 1;
     const int max_splits = env_int("B200TRK_TC_SPLITK", 1) ? 64 : 1;
-    const int slots = net->sms * (occ >= 2 ? 2 : 1);
+    const int slots = net->sms;
     if (ctas < slots) {
         splits = slots / ctas;
         const int min_kb = env_int("B200TRK_TC_MINKB", 4);
@@ -693,7 +497,6 @@ static int tc_configure(b200trk_net* net, const Op& op, TcConv* tc, int S) {
     P.splits = (P.total_kb + P.kb_per_split - 1) / P.kb_per_split;
     B200_REQUIRE(ctas <= 512 || P.splits == 1, "tc_conv: counter array too small for %d tiles", ctas);
     P.ws = op.side ? net->splitk_ws2 : net->splitk_ws;
-    { int need = acc_cols + (P.a_tmem ? P.stages * 64 : 0), cols = 32; while (cols < need) cols <<= 1; P.tmem_cols = cols; }
     P.cluster_red = (env_int("B200TRK_TC_CLUSTER", 1) && P.splits > 1 && P.splits <= 8) ? 1 : 0;
     P.prefetch_b = env_int("B200TRK_TC_PREFETCH_B", 1);
     const size_t Kt = (size_t)op.k * op.k * op.Cin;
@@ -708,18 +511,18 @@ int tc_conv_launch(b200trk_net* net, const Op& op, int S, cudaStream_t st) {
         if (int e = tc_configure(net, op, tc, S)) return e;
     const TcParams& P = tc->P;
     size_t smem = (size_t)P.stages * P.stage_bytes + 1024;
-    if (smem < 72 * 1024) smem = 72 * 1024;       // the epilogue stages accumulator rows in the (idle) pipeline buffers: up to 128 x 132 floats
-    static const int cw = env_int("B200TRK_TC_CW", 8) == 4 ? 4 : 8;
+    const size_t staging = (size_t)TC_BM * (P.BN + 4) * sizeof(float) + 1024;    // the epilogue's accumulator tile
+    if (smem < staging) smem = staging;
     static bool attr = false;
     if (!attr) {
-        B200_CHECK_CUDA(cudaFuncSetAttribute(conv_tc_kernel<4>, cudaFuncAttributeMaxDynamicSharedMemorySize, 220 * 1024));
-        B200_CHECK_CUDA(cudaFuncSetAttribute(conv_tc_kernel<8>, cudaFuncAttributeMaxDynamicSharedMemorySize, 220 * 1024));
+        B200_CHECK_CUDA(cudaFuncSetAttribute(conv_tc_kernel<64>, cudaFuncAttributeMaxDynamicSharedMemorySize, TC_SMEM_MAX));
+        B200_CHECK_CUDA(cudaFuncSetAttribute(conv_tc_kernel<128>, cudaFuncAttributeMaxDynamicSharedMemorySize, TC_SMEM_MAX));
         attr = true;
     }
     dim3 grid(P.tiles_w * P.tiles_h * S, op.Cout / P.BN, P.splits);
     cudaLaunchConfig_t cfg;
     memset(&cfg, 0, sizeof(cfg));
-    cfg.gridDim = grid; cfg.blockDim = dim3(64 + 32 * cw); cfg.dynamicSmemBytes = smem; cfg.stream = st;
+    cfg.gridDim = grid; cfg.blockDim = dim3(TC_THREADS); cfg.dynamicSmemBytes = smem; cfg.stream = st;
     cudaLaunchAttribute at[2];
     int nat = 0;
     static const int use_pdl = env_int("B200TRK_TC_PDL", 1);
@@ -734,8 +537,8 @@ int tc_conv_launch(b200trk_net* net, const Op& op, int S, cudaStream_t st) {
         ++nat;
     }
     cfg.attrs = at; cfg.numAttrs = nat;
-    if (cw == 4) B200_CHECK_CUDA(cudaLaunchKernelEx(&cfg, conv_tc_kernel<4>, P));
-    else B200_CHECK_CUDA(cudaLaunchKernelEx(&cfg, conv_tc_kernel<8>, P));
+    if (P.BN == 64) B200_CHECK_CUDA(cudaLaunchKernelEx(&cfg, conv_tc_kernel<64>, P));
+    else B200_CHECK_CUDA(cudaLaunchKernelEx(&cfg, conv_tc_kernel<128>, P));
     B200_LAUNCH_CHECK();
     return 0;
 }
@@ -744,7 +547,6 @@ void tc_conv_free(TcConv* tc) { delete tc; }
 
 int tc_conv_set_debug(Op& op, unsigned long long* buf) {
     op.tc->P.dbg = buf;
-    op.tc->P.trace = buf ? buf + 8 * 2048 : nullptr;     // second half of the [4096][8] debug buffer
     return 0;
 }
 int tc_conv_grid(const Op& op, int dims[4]) {

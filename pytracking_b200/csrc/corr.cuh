@@ -2,13 +2,13 @@
 // sample memories -- the two data sweeps of stages 2 and 3 (SURVEY.md 9.1):
 //     apply:      s[i,y,x]  = sum_{c,u,v} xpad[i,c,y+u,x+v] * w[c,u,v]
 //     transpose:  g[c,u,v]  = sum_{i,y,x} r[i,y,x] * xpad[i,c,y+u,x+v]
-// Both are 5776 MAC per (sample, channel) over a 324-float plane: ~9 FLOP/B, i.e. right at the B200
-// fp32-FMA : HBM balance point, so the kernels must be FMA-efficient AND stream each plane exactly once.
+// Both are 5776 MAC per (sample, channel) over a 324-float plane: ~9 FLOP/B, under the H100's fp32-FMA : HBM balance point
+// (~20 FLOP/B by the data sheet), so the kernels must stream each plane exactly once and stay FMA-efficient.
 //
 // Work decomposition inside a CTA: a "slot" is one channel plane staged zero-padded in shared memory; the
 // (FS+1)^2 outputs are cut into 5x4 register tiles; thread = (slot, tile).  Per channel a thread reads an
 // 8x7 input patch (56 LDS) and issues 320 FMAs (5.7 FMA per shared-memory word, above the 4:1 needed to
-// be FMA-bound on sm_100).  Planes are double-buffered: the next item's planes are fetched with coalesced
+// be FMA-bound).  Planes are double-buffered: the next item's planes are fetched with coalesced
 // 128-bit global loads into registers while the current one is being consumed.
 #pragma once
 #include "common.cuh"

@@ -10,7 +10,7 @@
 //   b      = yf conj(sum_n sw_n X_n),   M1 r = r / diag_M   (diag_M real, from the running sample energy)
 //   <a,b>  = sum over the half spectrum, kx = 0 once and kx > 0 twice (fourier.inner_prod_fs)
 //
-// Design (B200): the data term is local to a Fourier coefficient -- a [N, C] complex slab of the sample memory
+// Design: the data term is local to a Fourier coefficient -- a [N, C] complex slab of the sample memory
 // [H, Wh, N, C, 2] times a C-vector and back -- so the coefficients are dealt to the CTAs in contiguous ranges and every CTA keeps
 // as many of its slabs as fit RESIDENT IN SHARED MEMORY for the whole call (deep block: 15x8 coefficients x 200 x 64 x 8 B =
 // 102 KB per coefficient, one per SM; shallow block: 25.6 KB slabs, 8 of a CTA's ~14 resident, the rest stream from L2):

@@ -1,5 +1,5 @@
 // Shared by the two implementations of the steepest-descent optimisers: sd_optimizer.cu (fp32 CUDA-core sweeps, any C / n)
-// and sd_tc.cu (tcgen05 sweeps; C a multiple of 128).
+// and sd_tc.cu (wgmma sweeps; C a multiple of 128).
 #pragma once
 #include "common.cuh"
 
@@ -45,7 +45,7 @@ __device__ __forceinline__ float lut_lerp(const float* lut, int nb, float rho) {
     return lut[b] * (1.f - f) + lut[b + 1] * f;
 }
 
-// tcgen05 path (sd_tc.cu). Returns 0 and sets *handled = 1 when it ran; *handled = 0 when the shape is not claimed (the
+// Tensor-core path (sd_tc.cu). Returns 0 and sets *handled = 1 when it ran; *handled = 0 when the shape is not claimed (the
 // caller then uses the CUDA-core kernel); non-zero status on error.
 template <int FS, int MODE>
 int launch_sd_tc(const SdParams& P, cudaStream_t st, int* handled);

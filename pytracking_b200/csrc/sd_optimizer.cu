@@ -42,7 +42,7 @@ static int launch_sd(SdParams P, cudaStream_t st) {
         if (handled) return 0;
     }
     // Decomposition: passes x 16 channels per CTA (NCH chunks) x NG sample groups. The sweep time is set by the busiest CTA,
-    // ceil(n / NG) * passes items, so every admissible `passes` is scored (n = 50 on 148 SMs: 4 passes -> 8 items, 2 -> 6).
+    // ceil(n / NG) * passes items, so every admissible `passes` is scored.
     const int sms = device_sm_count();
     const size_t limit = 227 * 1024 - 512;
     const size_t item = (size_t)K::ITEM_FLOATS * sizeof(float);

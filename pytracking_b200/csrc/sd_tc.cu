@@ -1,16 +1,17 @@
 // Stage 3 on the tensor cores: the steepest-descent optimisers (same four modes and the same algebra as sd_optimizer.cu)
-// with both sweeps over the sample memory issued as tcgen05 GEMMs with a 16-wide N (the 16 filter taps):
+// with both sweeps over the sample memory issued as Hopper warpgroup MMAs (wgmma, M = 64 per warpgroup) with a 16-wide N (the
+// 16 filter taps):
 //
 //   adjoint sweep   g[c, tap]  = sum_{i, p} X_i[c, p] * R_i[p, tap]        R_i[p, tap] = r_i[p shifted by the tap]   (A^T r)
-//       A = X_i[128 channels x 32 pixels]  (K-major straight from the [n, C, H*W] sample memory, TMA box)
-//       B = R_i^T[16 taps x 32 pixels]      (gathered from the residual map in shared memory by the converter warps)
+//       A = X_i[128 channels x 32 pixels]  (K-major straight from the [n, C, H*W] sample memory, TMA box, 128-byte swizzle)
+//       B = R_i^T[16 taps x 32 pixels]      (gathered from the residual map by the consumer threads into the stage)
 //   apply sweep     T_i[p, tap] = sum_c X_i[p, c] * F[c, tap] ;  s_i[y, x] = sum_tap T_i[(y, x) shifted by the tap, tap]   (A f)
-//       A = X_i[128 pixels x 32 channels]  (the SAME [n, C, H*W] memory: the TMA box is 32 channel rows x 128 pixels and the
-//                                            converter warps transpose it on the way into tensor memory)
+//       A = X_i[128 pixels x 32 channels]  (the SAME [n, C, H*W] memory: the TMA box is 32 channel rows x 128 pixels; TF32 wgmma
+//                                            wants K-major operands, so A is read transposed from shared memory into registers)
 //       B = F^T[16 taps x 32 channels]      (the filter / gradient, resident in shared memory for the whole sweep)
 //
-// fp32 fidelity as in conv_tc.cu: every operand is split x = hi + lo with hi = the TF32 truncation the datapath applies anyway,
-// three MMAs per K step (A_lo*B_hi, A_hi*B_lo, A_hi*B_hi), each product into its own fp32 TMEM accumulator (summed in the epilogue).
+// fp32 fidelity as in conv_tc.cu: every operand is split x = hi + lo (both TF32, round to nearest), three MMAs per K step
+// (A_lo*B_hi + A_hi*B_lo into one fp32 register accumulator, A_hi*B_hi into another; summed in the epilogue).
 //
 // Work decomposition: a "unit" is one 128 x 32 operand tile (16 KB of sample memory). The units of a sweep are numbered
 // (adjoint: chunk, sample, pixel block; apply: sample, pixel tile, channel block) and CTA b of G takes the contiguous range
@@ -24,18 +25,12 @@
 // `smax`); the replicas evolve identically because all of them read the same partials in the same order; loss / curvature
 // terms are contributed by the sample's owner (the CTA holding its first unit) only.
 //
-// Operand pipeline (per unit): TMA lands the raw 128 x 32 fp32 tile in a shared-memory stage; a converter thread reads its operand row
-// back (conflict-free through the 128-byte swizzle) and writes hi (= raw) and lo straight into a TENSOR-MEMORY stage with tcgen05.st;
-// the MMAs take A from TMEM (tcgen05.mma with a TMEM A operand) and only the 16-row B operand from shared memory. The shared-memory
-// stage is free again as soon as it has been read (not when the MMAs retire), so 6 x 20 KB stages cover the L2 latency, and the
-// shared-memory traffic per unit is 16 KB in + 16 KB out instead of ~100 KB.
-//
-// Warp roles during a sweep: warp 0 = TMA producer (it also issues the first units of the NEXT sweep while the CTAs sit in the grid
-// barrier), warps 1 / 10 / 11 = MMA issuers (one per product), warps 2-5 and 6-9 = two converter groups that take ALTERNATE units (the
-// per-unit chain wait -> read -> tcgen05.st -> publish is latency, so two chains in flight double the unit rate) and share the
-// segment epilogues (TMEM -> registers -> partials). All 384 threads run the element-wise phases between the sweeps. Every role walks
-// its units with running counters (no integer division per unit). Measured stage times and what paces the sweeps: DESIGN.md sections
-// 4.1b and 8, profiles/r02{n,o,p}_sd_tc_units.txt (round 1: profiles/r01j_sd_tc_pipeline.txt).
+// Operand pipeline (per unit): warp 8 (the producer) lands the raw 128 x 32 fp32 tile in one of up to 8 shared-memory stages with
+// TMA; warps 0-7 (two consumer warpgroups, rows 0-63 / 64-127 of the tile) read their A fragments into registers, split them, and
+// issue 4 K steps x 3 products as register-A wgmmas against the 16-row B operand in shared memory. The apply sweep frees a stage
+// as soon as its fragments are in registers; the adjoint sweep also stages the unit's B tile there and frees it when the MMAs have
+// retired. The producer also issues the first units of the NEXT sweep while the CTAs sit in the grid barrier. All 288 threads
+// run the element-wise phases between the sweeps.
 #include "tc_ptx.cuh"
 #include "sd_common.cuh"
 #include <atomic>
@@ -44,12 +39,10 @@
 
 namespace b200trk {
 
-constexpr int STC_THREADS = 384;              // warp 0 producer, 1 / 10 / 11 MMA issuers, 2-9 converters + epilogue
-constexpr int STC_CT = 256;                 // converter / epilogue threads (warps 2..9)
-constexpr int STC_NS_MAX = 8;               // shared-memory stages (runtime count Q.ns >= STC_NT)
-constexpr int STC_NT = 4;                   // tensor-memory stages: 64 columns each (32 hi + 32 lo)
-constexpr int STC_ACC_COL = STC_NT * 64;    // accumulators behind the operand stages
-constexpr int STC_TMEM_COLS = 512;
+constexpr int STC_CT = 256;                 // consumer threads (warps 0-7: two warpgroups)
+constexpr int STC_THREADS = STC_CT + 32;    // + warp 8, the TMA producer
+constexpr int STC_NS_MAX = 8;               // shared-memory stages (runtime count Q.ns)
+constexpr int STC_NS_MIN = 4;
 constexpr int STC_A_BYTES = 16384;          // 128 rows x 128 B
 constexpr int STC_STAGE_BYTES = 20480;      // A raw | B_hi (2 KB) | B_lo (2 KB)
 constexpr int STC_MAXCH = 4;                // 128-channel chunks (C <= 512)
@@ -69,14 +62,7 @@ struct SdTcParams {
 __device__ __forceinline__ int part_lo(long long U, int G, int b) { return (int)((U * (long long)b) / G); }
 __device__ __forceinline__ int part_owner(long long U, int G, int u) { return (int)((((long long)u + 1) * G - 1) / U); }
 
-// non-blocking phase test (acquire): true once the phase with the given parity has completed
-__device__ __forceinline__ bool mbar_test(uint32_t bar, uint32_t parity) {
-    uint32_t ok;
-    asm volatile("{\n\t.reg .pred p;\n\tmbarrier.test_wait.parity.shared::cta.b64 p, [%1], %2;\n\tselp.u32 %0, 1, 0, p;\n\t}"
-                 : "=r"(ok) : "r"(bar), "r"(parity) : "memory");
-    return ok != 0;
-}
-__device__ __forceinline__ float lo_trunc(float x) { return x - __uint_as_float(__float_as_uint(x) & 0xffffe000u); }
+__device__ __forceinline__ float tf32_lo(float x) { return tf32_rna(x - tf32_rna(x)); }
 // byte offset of element (row, k) inside a K-major SWIZZLE_128B tile of 128-byte rows (tile base 1024-byte aligned)
 __device__ __forceinline__ uint32_t sw128(int row, int k) {
     return (uint32_t)(row * 128 + ((((k >> 2) ^ (row & 7)) << 4) | ((k & 3) << 2)));
@@ -96,11 +82,7 @@ __global__ void __launch_bounds__(STC_THREADS, 1) sd_tc_kernel(const __grid_cons
     constexpr int NTH = STC_THREADS;
     extern __shared__ uint8_t stc_raw[];
     __shared__ __align__(8) uint64_t s_full[STC_NS_MAX];      // TMA landed the raw tile in shared-memory stage s
-    __shared__ __align__(8) uint64_t s_sfree[STC_NS_MAX];     // the converter warps have read stage s
-    __shared__ __align__(8) uint64_t s_tready[STC_NT];        // hi / lo of a unit are in tensor-memory stage t (+ its B tile in smem)
-    __shared__ __align__(8) uint64_t s_tfree[STC_NT];         // the MMAs reading tensor-memory stage t have retired
-    __shared__ __align__(8) uint64_t s_acc;
-    __shared__ uint32_t s_tmem;
+    __shared__ __align__(8) uint64_t s_sfree[STC_NS_MAX];     // the consumer warps are done with stage s
     __shared__ float s_red[32];
     __shared__ float s_scal[4];
     __shared__ int s_state[16];        // sample ids of the state slots
@@ -141,9 +123,7 @@ __global__ void __launch_bounds__(STC_THREADS, 1) sd_tc_kernel(const __grid_cons
     SD_STAMP(0);
     // ---- prologue ------------------------------------------------------------------------------------------------------------
     if (tid == 0) {
-        for (int i = 0; i < NS; ++i) { mbar_init(smem_u32(&s_full[i]), 1); mbar_init(smem_u32(&s_sfree[i]), STC_CT / 64); }
-        for (int i = 0; i < STC_NT; ++i) { mbar_init(smem_u32(&s_tready[i]), STC_CT / 64); mbar_init(smem_u32(&s_tfree[i]), 3); }
-        mbar_init(smem_u32(&s_acc), 3);
+        for (int i = 0; i < NS; ++i) { mbar_init(smem_u32(&s_full[i]), 1); mbar_init(smem_u32(&s_sfree[i]), STC_CT / 32); }
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
         // state slots: the samples of this CTA's adjoint range (runs of KBT units per (chunk, sample))
         int ns = 0;
@@ -160,11 +140,7 @@ __global__ void __launch_bounds__(STC_THREADS, 1) sd_tc_kernel(const __grid_cons
         }
         s_ns = ns;
     }
-    if (warp == 1) {
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(&s_tmem)), "r"((uint32_t)STC_TMEM_COLS) : "memory");
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-    }
-    if (warp == 0 && lane == 0) {
+    if (warp == 8 && lane == 0) {
         asm volatile("prefetch.tensormap [%0];" ::"l"((uint64_t)&Q.map_t) : "memory");
         asm volatile("prefetch.tensormap [%0];" ::"l"((uint64_t)&Q.map_a) : "memory");
     }
@@ -175,10 +151,7 @@ __global__ void __launch_bounds__(STC_THREADS, 1) sd_tc_kernel(const __grid_cons
         s_bf[tid] = part_owner(UT, G, tid * per_chunk);
         s_bl[tid] = part_owner(UT, G, (tid + 1) * per_chunk - 1);
     }
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem = __shfl_sync(0xffffffffu, s_tmem, 0);      // provably warp-uniform (see tc_ptx.cuh)
     const int ns = s_ns;
 
     // valid apply-segment slots of every state sample: a segment starts at channel block 0 of a (sample, pixel tile) run and at
@@ -255,12 +228,12 @@ __global__ void __launch_bounds__(STC_THREADS, 1) sd_tc_kernel(const __grid_cons
     }
 
     // ---- helpers -------------------------------------------------------------------------------------------------------------
-    uint32_t ucount = 0, acount = 0;    // units / accumulator commits so far (identical in every thread)
+    uint32_t ucount = 0;                // units so far (identical in every thread)
     unsigned epoch = 0;
-    const uint32_t idesc = (1u << 4) | (2u << 7) | (2u << 10) | ((uint32_t)(16 >> 3) << 17) | ((uint32_t)(128 >> 4) << 24);
-    const int q = warp & 3, half = (warp - 2) >> 2;                  // converter warps: TMEM lane quadrant; conversion group / epilogue column half
-    const int grp = half;
-    const int ct = tid - 64;
+    // consumer fragment coordinates (wgmma m64n16k8): rows r0, r0 + 8 of the tile, K column kq (+4), accumulator columns 8j + 2kq (+1)
+    const int wg = warp >> 2;
+    const int r0 = wg * 64 + (warp & 3) * 16 + (lane >> 2), kq = lane & 3;
+    const int ct = tid;                                               // consumer thread 0..255
 
     // F^T (hi | lo) of all channel blocks from a [C][16] vector in global memory
     auto build_ft = [&](const float* src) {
@@ -281,8 +254,8 @@ __global__ void __launch_bounds__(STC_THREADS, 1) sd_tc_kernel(const __grid_cons
 #pragma unroll
                     for (int k = 0; k < 4; ++k) {
                         uint8_t* t = ftb + (size_t)(c >> 5) * 4096 + sw128(tap0 + k, c & 31);
-                        *reinterpret_cast<float*>(t) = e[k];
-                        *reinterpret_cast<float*>(t + 2048) = lo_trunc(e[k]);
+                        *reinterpret_cast<float*>(t) = tf32_rna(e[k]);
+                        *reinterpret_cast<float*>(t + 2048) = tf32_lo(e[k]);
                     }
                 }
             }
@@ -292,121 +265,63 @@ __global__ void __launch_bounds__(STC_THREADS, 1) sd_tc_kernel(const __grid_cons
     };
 
     // per-unit pipeline stamps (SM clock) of CTA 0 during the first adjoint sweep: utr[unit][16]
-    // 0 slot free (producer) 1 TMA issued | 8 converter reaches the unit 2 tile landed 3 TMEM stage free 9 operands in registers 4 tcgen05.st
-    // retired 5 published | 6 MMA warp sees the unit 7 MMAs + commit issued
+    // 0 slot free (producer) 1 TMA issued | 2 tile landed (consumer) 9 operands in registers 7 MMAs retired 5 stage released
     long long* utr = nullptr;
     int utr_i = 0;
 #define UTR(k) do { if (utr && utr_i < 16) utr[utr_i * 16 + (k)] = clock64(); } while (0)
     // ---- operand pipeline pieces --------------------------------------------------------------------------------------------
-    // Every role walks the units of a sweep with RUNNING stage counters and unit coordinates (no integer division per unit: the
-    // per-unit index arithmetic with run-time divisors cost the converter warps several hundred cycles per unit and, not the TMA
-    // unit, paced the sweeps: profiles/r02n_sd_tc_units.txt).  ug = units since kernel start; shared-memory stage = ug % NS with
-    // parity (ug / NS) & 1, tensor-memory stage = ug % 4 with parity (ug / 4) & 1.
-    struct Stage { uint32_t s, sp, t, tp; };
-    auto stage_of = [&](uint32_t ug) { Stage g; g.s = ug % (uint32_t)NS; g.sp = (ug / (uint32_t)NS) & 1u; g.t = ug % STC_NT; g.tp = (ug / STC_NT) & 1u; return g; };
-    auto stage_next = [&](Stage& g) {
-        if (++g.s == (uint32_t)NS) { g.s = 0; g.sp ^= 1u; }
-        if (++g.t == (uint32_t)STC_NT) { g.t = 0; g.tp ^= 1u; }
-    };
+    // Every role walks the units of a sweep with RUNNING stage counters and unit coordinates (no integer division per unit).
+    // ug = units since kernel start; shared-memory stage = ug % NS with parity (ug / NS) & 1.
+    struct Stage { uint32_t s, sp; };
+    auto stage_of = [&](uint32_t ug) { Stage g; g.s = ug % (uint32_t)NS; g.sp = (ug / (uint32_t)NS) & 1u; return g; };
+    auto stage_next = [&](Stage& g) { if (++g.s == (uint32_t)NS) { g.s = 0; g.sp ^= 1u; } };
     // producer: raw tile of one unit -> shared-memory stage g.s
     auto produce = [&](const Stage& g, const CUtensorMap* map, int c0, int c1, int c2) {
         mbar_wait(smem_u32(&s_sfree[g.s]), g.sp ^ 1u);
         if (lane == 0) UTR(0);
         const uint32_t full = smem_u32(&s_full[g.s]);
-        if (P.dbg_mode == 4 || (P.dbg_mode == 5 && (blockIdx.x & 1))) {
-            // timing experiments (results are garbage): 4 = no TMA traffic, 5 = only every second CTA loads
-            mbar_arrive_elect(full);
-            return;
-        }
         mbar_expect_tx_elect(full, STC_A_BYTES);
         tma_load_3d_elect(base_u32 + g.s * STC_STAGE_BYTES, map, full, c0, c1, c2);
         if (lane == 0) UTR(1);
     };
-    // converter: the eight converter warps form TWO groups of four (grp 0 = warps 2-5, grp 1 = warps 6-9; a group covers the four
-    // TMEM lane quadrants) and the groups take alternate units of a sweep: the per-unit chain of barrier waits, shared-memory
-    // reads, tensor-memory stores and the publish step is latency, not throughput, so two independent chains double the unit rate
-    // (profiles/r02o_sd_tc_units.txt).  Thread = operand row: wait for the tile and for the tensor-memory stage, then 2 x (16 fp32 of
-    // the row -> hi (raw: the datapath truncates) and lo -> tcgen05.st).  Returns the shared-memory stage (for the adjoint sweep's B tile).
-    // have_full / have_tfree: the group already saw the two barriers complete (non-blocking tests issued one unit ahead, see
-    // `lookahead`), so the ~2 x 170-cycle blocking waits drop out of the chain whenever the pipeline runs ahead of the converters.
-    auto convert_unit = [&](const Stage& g, bool transposed, bool have_full, bool have_tfree) -> uint8_t* {
-        if (!have_full) mbar_wait(smem_u32(&s_full[g.s]), g.sp);
-        if (ct == 0) UTR(2);
-        if (!have_tfree) mbar_wait(smem_u32(&s_tfree[g.t]), g.tp ^ 1u);
-        tc_fence_after();
-        if (ct == 0) UTR(3);
-        uint8_t* sb = base + (size_t)g.s * STC_STAGE_BYTES;
-        if (P.dbg_mode == 3) return sb;     // timing experiment: no operand conversion
-        const int row = q * 32 + lane;
-        const uint8_t* arow = sb + row * 128;
-        const uint32_t ta = tmem + ((uint32_t)(q * 32) << 16) + g.t * 64u;
-        // all 32 elements of the row first (the tensor-memory stores below are ordered asm statements: loads issued after them would
-        // wait for them), then hi / lo of each half row
-        float x[32];
-        if (!transposed) {
-            // tile = [128 rows][32 k] with the 128-byte swizzle: this thread's row
+    // consumer: this thread's A fragments of the unit (4 K steps x 4 registers), split into hi / lo
+    auto load_frags = [&](const uint8_t* sb, bool transposed, uint32_t (&ah)[4][4], uint32_t (&al)[4][4]) {
+        float x[4][4];
 #pragma unroll
-            for (int j = 0; j < 8; ++j) {
-                const float4 v = *reinterpret_cast<const float4*>(arow + ((j ^ (row & 7)) << 4));
-                x[4 * j] = v.x; x[4 * j + 1] = v.y; x[4 * j + 2] = v.z; x[4 * j + 3] = v.w;
+        for (int ks = 0; ks < 4; ++ks) {
+#pragma unroll
+            for (int r = 0; r < 4; ++r) {
+                const int row = r0 + 8 * (r & 1), k = 8 * ks + kq + 4 * (r >> 1);
+                // adjoint: [128 rows][32 k] with the 128-byte swizzle; apply: [32 k][128 rows] linear (512-byte lines)
+                x[ks][r] = transposed ? reinterpret_cast<const float*>(sb)[k * 128 + row] : *reinterpret_cast<const float*>(sb + sw128(row, k));
             }
-        } else {
-            // tile = [32 k][128 rows] linear (512-byte lines): the lanes of a warp read 32 consecutive words of one line
-            const float* col = reinterpret_cast<const float*>(sb) + row;
-#pragma unroll
-            for (int j = 0; j < 32; ++j) x[j] = col[j * 128];
         }
 #pragma unroll
-        for (int hh = 0; hh < 2; ++hh) {
-            uint32_t hi[16], lo[16];
+        for (int ks = 0; ks < 4; ++ks)
 #pragma unroll
-            for (int j = 0; j < 16; ++j) { hi[j] = __float_as_uint(x[hh * 16 + j]); lo[j] = __float_as_uint(lo_trunc(x[hh * 16 + j])); }
-            tmem_st16(ta + (uint32_t)(hh * 16), hi);
-            tmem_st16(ta + 32u + (uint32_t)(hh * 16), lo);
+            for (int r = 0; r < 4; ++r) {
+                float h, l;
+                split_tf32(x[ks][r], h, l);
+                ah[ks][r] = __float_as_uint(h); al[ks][r] = __float_as_uint(l);
+            }
+    };
+    // consumer: the three products of one unit against the B tile at b_hi (B_lo 2 KB behind it), then wait for them to retire
+    auto mma_unit = [&](float (&acc)[8], float (&acc2)[8], const uint32_t (&ah)[4][4], const uint32_t (&al)[4][4], uint32_t b_hi) {
+        wgmma_fence();
+#pragma unroll
+        for (int ks = 0; ks < 4; ++ks) {
+            const uint64_t dh = wg_desc(b_hi + (uint32_t)ks * 32u), dl = wg_desc(b_hi + 2048u + (uint32_t)ks * 32u);
+            wgmma_rs_n16(acc2, al[ks], dh);
+            wgmma_rs_n16(acc2, ah[ks], dl);
+            wgmma_rs_n16(acc, ah[ks], dh);
         }
-        if (ct == 0) UTR(9);
-        return sb;
+        wgmma_commit();
+        wgmma_wait<0>();
+        wg_reg_fence(acc); wg_reg_fence(acc2);
     };
-    // barrier tests for the group's NEXT unit, issued between the tensor-memory stores of the current unit and their retirement
-    // (A parity test is only meaningful while the barrier is at most one phase behind.  s_tfree: the previous user of the stage is
-    //  this group's own unit i - 2, and the MMAs retire in order.  s_full: the previous user of the stage is unit i + 2 - NS, this
-    //  group's own (already converted) unit when NS is even; with an odd stage count it belongs to the other group and its tile is
-    //  not known to have landed, so the test is not used.)
-    auto lookahead = [&](const Stage& g2, bool& have_full, bool& have_tfree) {
-        if (P.dbg_mode == 7) { have_full = have_tfree = false; return; }       // timing experiment: blocking waits only
-        have_full = ((NS & 1) == 0) && mbar_test(smem_u32(&s_full[g2.s]), g2.sp);
-        have_tfree = mbar_test(smem_u32(&s_tfree[g2.t]), g2.tp ^ 1u);
-    };
-    // converter, last step: publish the unit (shared-memory stage free again, tensor-memory stage ready); one arrival per warp of the group
-    auto publish = [&](const Stage& g) {
-        asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory");
-        if (ct == 0) UTR(4);
-        tc_fence_before();
+    auto release = [&](const Stage& g) {
         __syncwarp();
-        if (lane == 0) {
-            asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(&s_sfree[g.s])) : "memory");
-            asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(&s_tready[g.t])) : "memory");
-        }
-        if (ct == 0) UTR(5);
-    };
-    // MMA issuers: three warps (1, 10, 11), one per product of the 3xTF32 expansion (A_lo*B_hi, A_hi*B_lo, A_hi*B_hi), each into
-    // its own 16-column accumulator (acc + 16 * prod); issuing a tcgen05.mma costs one warp ~100 cycles of scalar work, so a single
-    // issue warp (12 MMAs per unit) was the slowest stage of the pipeline. A = tensor-memory stage t, B from shared memory.
-    const int prod = (warp == 1) ? 0 : warp - 9;
-    auto issue = [&](const Stage& g, uint32_t acc, uint32_t b_hi_addr, bool first) {
-        mbar_wait(smem_u32(&s_tready[g.t]), g.tp);
-        tc_fence_after();
-        if (lane == 0 && prod == 0) UTR(6);
-        const uint32_t a_op = tmem + g.t * 64u + ((prod == 0) ? 32u : 0u);                             // lo | hi | hi
-        const uint32_t d_b = make_smem_desc_lo(b_hi_addr) + ((prod == 1) ? (2048u >> 4) : 0u);       // hi | lo | hi
-        if (P.dbg_mode != 1 && !(P.dbg_mode == 2 && prod != 2)) {     // (timing experiments: 1 = no MMAs, 2 = hi*hi only)
-#pragma unroll
-            for (int k = 0; k < 4; ++k)
-                tc_mma_tf32_ts_lo(acc + (uint32_t)(16 * prod), a_op + (uint32_t)(k * 8), d_b + (uint32_t)(k * 32 >> 4), idesc,
-                                  (first && k == 0) ? 0u : 1u);
-        }
-        tc_commit_elect(smem_u32(&s_tfree[g.t]));
-        if (lane == 0 && prod == 0) UTR(7);
+        if (lane == 0) mbar_arrive(smem_u32(&s_sfree[g.s]));
     };
 
     // unit coordinates: adjoint sweep (chunk, sample, pixel block), apply sweep (sample, pixel tile, channel block)
@@ -422,7 +337,7 @@ __global__ void __launch_bounds__(STC_THREADS, 1) sd_tc_kernel(const __grid_cons
     // shared-memory stages); those tiles land while the CTAs sit in the grid barriers / reductions between the sweeps.
     // pf_apply / pf_adj = units of the coming apply / adjoint sweep already issued.
     int pf_apply = 0, pf_adj = 0;
-    const bool xpf = (P.dbg_mode != 6);
+    const bool xpf = true;
     auto produce_apply_run = [&](uint32_t ug, int i0, int i1) {        // units i0 .. i1-1 of this CTA's apply range; ug = global index of i0
         if (i0 >= i1) return;
         Stage g = stage_of(ug);
@@ -446,78 +361,62 @@ __global__ void __launch_bounds__(STC_THREADS, 1) sd_tc_kernel(const __grid_cons
     // apply sweep: qslots[segment] = shift-added partial map of every (sample, pixel tile) segment of this CTA's range
     auto sweep_apply = [&](bool adjoint_follows) {
         const int nun = a_hi - a_lo;
-        int nseg = 0;
-        { int kb = (nun > 0) ? a_lo % kba : 0; for (int i = 0; i < nun; ++i) { nseg += (i == 0 || kb == 0) ? 1 : 0; if (++kb == kba) kb = 0; } }
         if (nun > 0) {
-            if (warp == 0) {
+            if (warp == 8) {
                 // (whole warp, converged: see tc_ptx.cuh)
                 produce_apply_run(ucount + (uint32_t)pf_apply, pf_apply, nun);
                 if (xpf && adjoint_follows) produce_adj_run(ucount + (uint32_t)nun, 0, min(NS, t_hi - t_lo), false);
-            } else if (warp == 1 || warp >= 10) {
-                int kb = a_lo % kba;
-                const uint32_t ftb_m = smem_u32(ftb);
-                Stage g = stage_of(ucount);
-                for (int i = 0; i < nun; ++i) {
-                    const bool seg_first = (i == 0 || kb == 0), seg_last = (i == nun - 1 || kb == kba - 1);
-                    issue(g, tmem + STC_ACC_COL, ftb_m + (uint32_t)kb * 4096u, seg_first);
-                    if (seg_last) tc_commit_elect(smem_u32(&s_acc));
-                    if (++kb == kba) kb = 0;
-                    stage_next(g);
-                }
             } else {
-                int seg = 0, kb_first = 0;
+                const uint32_t ftb_m = smem_u32(ftb);
+                int kb_first = 0;
                 Stage g = stage_of(ucount);
                 AppPos c = app_pos(a_lo);
-                bool have_full = false, have_tfree = false;
+                float acc[8], acc2[8];
+#pragma unroll
+                for (int i = 0; i < 8; ++i) { acc[i] = 0.f; acc2[i] = 0.f; }
                 for (int i = 0; i < nun; ++i) {
                     const bool seg_first = (i == 0 || c.kb == 0), seg_last = (i == nun - 1 || c.kb == kba - 1);
                     if (seg_first) kb_first = c.kb;
-                    if ((i & 1) == grp) {
-                        convert_unit(g, true, have_full, have_tfree);
-                        have_full = have_tfree = false;
-                        if (i + 2 < nun) { Stage g2 = g; stage_next(g2); stage_next(g2); lookahead(g2, have_full, have_tfree); }
-                        publish(g);
-                    }
+                    mbar_wait(smem_u32(&s_full[g.s]), g.sp);
+                    uint32_t ah[4][4], al[4][4];
+                    load_frags(base + (size_t)g.s * STC_STAGE_BYTES, true, ah, al);
+                    release(g);                                   // A is in registers, B (F^T) lives outside the stages
+                    mma_unit(acc, acc2, ah, al, ftb_m + (uint32_t)c.kb * 4096u);
                     if (seg_last) {
-                        // (both groups: the accumulator barrier completes only after every unit of the segment has been converted,
-                        //  published and multiplied, whichever group owned it)
-                        // T[p][tap] of the finished segment: TMEM -> Tt[tap][p] -> shift-add over the taps -> qslots
-                        mbar_wait(smem_u32(&s_acc), (acount + seg) & 1u);
-                        tc_fence_after();
-                        uint32_t v0[8], v1[8], v2[8];
-                        const uint32_t ta = tmem + ((uint32_t)(q * 32) << 16) + (uint32_t)(STC_ACC_COL + half * 8);
-                        tmem_ld8(ta, v0); tmem_ld8(ta + 16u, v1); tmem_ld8(ta + 32u, v2);
+                        // T[p][tap] of the finished segment: registers -> Tt[tap][p] -> shift-add over the taps -> qslots
 #pragma unroll
-                        for (int t = 0; t < 8; ++t)
-                            Tt[(half * 8 + t) * STC_TT_PITCH + q * 32 + lane] = (__uint_as_float(v0[t]) + __uint_as_float(v1[t])) + __uint_as_float(v2[t]);
-                        tc_fence_before();
+                        for (int j = 0; j < 2; ++j)
+#pragma unroll
+                            for (int h = 0; h < 2; ++h)
+#pragma unroll
+                                for (int e = 0; e < 2; ++e) {
+                                    const int t = 4 * j + 2 * h + e;
+                                    Tt[(8 * j + 2 * kq + e) * STC_TT_PITCH + r0 + 8 * h] = acc2[t] + acc[t];
+                                    acc[t] = 0.f; acc2[t] = 0.f;
+                                }
                         asm volatile("bar.sync 1, %0;" ::"n"(STC_CT) : "memory");
                         float* dst = Q.qslots + ((size_t)(c.smp * NPT + c.pt) * kba + kb_first) * NPOS;
                         for (int o = ct; o < NPOS; o += STC_CT) {
                             const int oy = o / OS, ox = o - oy * OS;
-                            float acc = 0.f;
+                            float sacc = 0.f;
 #pragma unroll
                             for (int tap = 0; tap < 16; ++tap) {
                                 const int iy = oy + (tap >> 2) - 2, ix = ox + (tap & 3) - 2;
                                 const int p = iy * FS + ix - c.pt * 128;
-                                if (iy >= 0 && iy < FS && ix >= 0 && ix < FS && p >= 0 && p < 128) acc += Tt[tap * STC_TT_PITCH + p];
+                                if (iy >= 0 && iy < FS && ix >= 0 && ix < FS && p >= 0 && p < 128) sacc += Tt[tap * STC_TT_PITCH + p];
                             }
-                            __stcg(dst + o, acc);
+                            __stcg(dst + o, sacc);
                         }
                         asm volatile("bar.sync 1, %0;" ::"n"(STC_CT) : "memory");
-                        ++seg;
                     }
                     stage_next(g); app_next(c);
                 }
             }
         }
         ucount += (uint32_t)nun;
-        acount += (uint32_t)nseg;
         pf_apply = 0;
         pf_adj = (xpf && adjoint_follows && nun > 0) ? min(NS, t_hi - t_lo) : 0;
-        tc_fence_before();
         __syncthreads();
-        tc_fence_after();
     };
 
     // adjoint sweep: gpart[b][local chunk][128][16] = partial gradient of this CTA's range
@@ -526,88 +425,74 @@ __global__ void __launch_bounds__(STC_THREADS, 1) sd_tc_kernel(const __grid_cons
         const int per_chunk = n * KBT;
         if (nun > 0) {
             const int chunk0 = t_lo / per_chunk;
-            if (warp == 0) {
+            if (warp == 8) {
                 produce_adj_run(ucount + (uint32_t)pf_adj, pf_adj, nun, true);
                 if (xpf) produce_apply_run(ucount + (uint32_t)nun, 0, min(NS, a_hi - a_lo));   // an apply sweep always follows an adjoint sweep
-            } else if (warp == 1 || warp >= 10) {
-                uint32_t touched = 0;
-                int cl = 0, left = (chunk0 + 1) * per_chunk - t_lo;      // units left in the current chunk
-                Stage g = stage_of(ucount);
-                for (int i = 0; i < nun; ++i) {
-                    utr_i = i;
-                    issue(g, tmem + (uint32_t)(STC_ACC_COL + cl * 48), base_u32 + g.s * STC_STAGE_BYTES + STC_A_BYTES,
-                          ((touched >> cl) & 1u) == 0u);
-                    touched |= 1u << cl;
-                    if (--left == 0) { ++cl; left = per_chunk; }
-                    stage_next(g);
-                }
-                tc_commit_elect(smem_u32(&s_acc));
             } else {
-                const int cg = ct & 127;                                 // thread index inside the group
-                const int tap = cg >> 3, kk0 = (cg & 7) * 4;             // this thread's four R^T elements: (tap, kk0 .. kk0 + 3)
+                const int tap = ct >> 4, kk0 = (ct & 15) * 2;             // this thread's two R^T elements: (tap, kk0 .. kk0 + 1)
                 const int dy = tap >> 2, dx = tap & 3;
-                const uint32_t boff = sw128(tap, kk0);                   // (kk0 is a multiple of 4: one 16-byte chunk of the swizzled row)
+                const uint32_t boff = sw128(tap, kk0);
                 Stage g = stage_of(ucount);
                 AdjPos c = adj_pos(t_lo);
-                if (grp == 1) { stage_next(g); adj_next(c); }           // group 1 owns the odd units
                 int j = 0, jsmp = -1;
-                float rv[4];
-                // this thread's four elements of R^T for the unit at `cc` (gathered from the mapped residual of the unit's sample)
-                auto gather = [&](const AdjPos& cc) {
-                    if (cc.smp != jsmp) {                               // state slot of the sample
-                        j = 0;
-                        for (int jj = 1; jj < ns; ++jj) j = (s_state[jj] == cc.smp) ? jj : j;
-                        jsmp = cc.smp;
-                    }
+                int cl = 0, left = (chunk0 + 1) * per_chunk - t_lo;      // units left in the current chunk
+                float acc[8], acc2[8];
 #pragma unroll
-                    for (int h = 0; h < 4; ++h) {
-                        const int px = cc.kb * 32 + kk0 + h;
+                for (int i = 0; i < 8; ++i) { acc[i] = 0.f; acc2[i] = 0.f; }
+                for (int i = 0; i < nun; ++i) {
+                    utr_i = i;
+                    // this thread's two elements of R^T for the unit (gathered from the mapped residual of the unit's sample)
+                    if (c.smp != jsmp) {                               // state slot of the sample
+                        j = 0;
+                        for (int jj = 1; jj < ns; ++jj) j = (s_state[jj] == c.smp) ? jj : j;
+                        jsmp = c.smp;
+                    }
+                    float rv[2];
+#pragma unroll
+                    for (int h = 0; h < 2; ++h) {
+                        const int px = c.kb * 32 + kk0 + h;
                         const int iy = px / FS, ix = px - iy * FS;
                         const int oy = iy - dy + 2, ox = ix - dx + 2;
                         rv[h] = (px < NPX && oy >= 0 && oy < OS && ox >= 0 && ox < OS) ? sT[j * NPOS + oy * OS + ox] : 0.f;
                     }
-                };
-                bool have_full = false, have_tfree = false;
-                if (grp < nun) gather(c);
-                for (int i = grp; i < nun; i += 2) {
-                    utr_i = i;
-                    if (ct == 0) UTR(8);
-                    // (the B area of the stage is free: the tfree wait / test covers the MMAs of unit ug - NS, NS >= NT)
-                    uint8_t* sb = convert_unit(g, false, have_full, have_tfree);
-                    *reinterpret_cast<float4*>(sb + STC_A_BYTES + boff) = make_float4(rv[0], rv[1], rv[2], rv[3]);
-                    *reinterpret_cast<float4*>(sb + STC_A_BYTES + 2048 + boff) = make_float4(lo_trunc(rv[0]), lo_trunc(rv[1]), lo_trunc(rv[2]), lo_trunc(rv[3]));
-                    asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-                    // while the tensor-memory stores of this unit retire: R^T elements and barrier tests of the group's next unit
-                    Stage g2 = g; stage_next(g2); stage_next(g2);
-                    AdjPos c2 = c; adj_next(c2); adj_next(c2);
-                    have_full = have_tfree = false;
-                    if (i + 2 < nun) { gather(c2); lookahead(g2, have_full, have_tfree); }
-                    publish(g);
-                    g = g2; c = c2;
-                }
-                mbar_wait(smem_u32(&s_acc), acount & 1u);
-                tc_fence_after();
-                const int ncl = (t_hi - 1) / per_chunk - chunk0 + 1;
-                for (int cl = 0; cl < ncl; ++cl) {
-                    uint32_t v0[8], v1[8], v2[8];
-                    const uint32_t ta = tmem + ((uint32_t)(q * 32) << 16) + (uint32_t)(STC_ACC_COL + cl * 48 + half * 8);
-                    tmem_ld8(ta, v0); tmem_ld8(ta + 16u, v1); tmem_ld8(ta + 32u, v2);
-                    float r[8];
+                    mbar_wait(smem_u32(&s_full[g.s]), g.sp);
+                    if (ct == 0) UTR(2);
+                    uint8_t* sb = base + (size_t)g.s * STC_STAGE_BYTES;
+                    float2 bh, bl;
+                    split_tf32(rv[0], bh.x, bl.x); split_tf32(rv[1], bh.y, bl.y);
+                    *reinterpret_cast<float2*>(sb + STC_A_BYTES + boff) = bh;
+                    *reinterpret_cast<float2*>(sb + STC_A_BYTES + 2048 + boff) = bl;
+                    uint32_t ah[4][4], al[4][4];
+                    load_frags(sb, false, ah, al);
+                    if (ct == 0) UTR(9);
+                    asm volatile("fence.proxy.async.shared::cta;" ::: "memory");   // B tile (generic-proxy writes) -> visible to wgmma
+                    asm volatile("bar.sync 1, %0;" ::"n"(STC_CT) : "memory");
+                    mma_unit(acc, acc2, ah, al, smem_u32(sb + STC_A_BYTES));
+                    if (ct == 0) UTR(7);
+                    release(g);
+                    if (ct == 0) UTR(5);
+                    if (--left == 0 || i == nun - 1) {
+                        // the chunk's partial gradient: rows = channels of the chunk, columns = taps
+                        float* dst = Q.gpart + ((size_t)b * STC_MAXCH + cl) * 128 * 16;
 #pragma unroll
-                    for (int t = 0; t < 8; ++t) r[t] = (__uint_as_float(v0[t]) + __uint_as_float(v1[t])) + __uint_as_float(v2[t]);
-                    float* dst = Q.gpart + (((size_t)b * STC_MAXCH + cl) * 128 + q * 32 + lane) * 16 + half * 8;
-                    __stcg(reinterpret_cast<float4*>(dst), make_float4(r[0], r[1], r[2], r[3]));
-                    __stcg(reinterpret_cast<float4*>(dst) + 1, make_float4(r[4], r[5], r[6], r[7]));
+                        for (int jj = 0; jj < 2; ++jj)
+#pragma unroll
+                            for (int h = 0; h < 2; ++h) {
+                                const int t = 4 * jj + 2 * h;
+                                __stcg(reinterpret_cast<float2*>(dst + (r0 + 8 * h) * 16 + 8 * jj + 2 * kq),
+                                       make_float2(acc2[t] + acc[t], acc2[t + 1] + acc[t + 1]));
+                                acc[t] = acc[t + 1] = acc2[t] = acc2[t + 1] = 0.f;
+                            }
+                        ++cl; left = per_chunk;
+                    }
+                    stage_next(g); adj_next(c);
                 }
             }
         }
         ucount += (uint32_t)nun;
-        acount += (nun > 0) ? 1u : 0u;
         pf_adj = 0;
         pf_apply = (xpf && nun > 0) ? min(NS, a_hi - a_lo) : 0;
-        tc_fence_before();
         __syncthreads();
-        tc_fence_after();
     };
 
     // q_j = sum of the apply-segment partial maps of state sample j, in slot order
@@ -826,12 +711,7 @@ __global__ void __launch_bounds__(STC_THREADS, 1) sd_tc_kernel(const __grid_cons
             }
         }
     }
-    tc_fence_before();
     __syncthreads();
-    if (warp == 1) {
-        tc_fence_after();
-        asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem), "r"((uint32_t)STC_TMEM_COLS) : "memory");
-    }
 }
 
 std::atomic<int> g_sd_last_tc{0};
@@ -870,7 +750,7 @@ int launch_sd_tc(const SdParams& P0, cudaStream_t st, int* handled) {
     const size_t fixed = 1024 + (size_t)kba * 4096 + 16 * STC_TT_PITCH * 4 + 2 * (size_t)slice_max * 16 +
                          (size_t)smax * 6 * NPOS * 4 + (size_t)smax * (STC_QL_MAX + 1) * 4 + 64;
     const size_t limit = 227 * 1024 - 3072;                     // static shared memory of the kernel: ~2.3 KB
-    if (fixed + (size_t)STC_NT * STC_STAGE_BYTES > limit) return 0;
+    if (fixed + (size_t)STC_NS_MIN * STC_STAGE_BYTES > limit) return 0;
     int nstg = (int)((limit - fixed) / STC_STAGE_BYTES);
     if (nstg > STC_NS_MAX) nstg = STC_NS_MAX;
     const size_t smem = fixed + (size_t)nstg * STC_STAGE_BYTES;
@@ -879,7 +759,6 @@ int launch_sd_tc(const SdParams& P0, cudaStream_t st, int* handled) {
     SdTcParams Q;
     memset(&Q, 0, sizeof(Q));
     Q.p = P0;
-    { const char* v = getenv("B200TRK_SD_DBG"); Q.p.dbg_mode = v ? atoi(v) : 0; }
     Q.p.trace = getenv("B200TRK_SD_TRACE") ? (unsigned long long*)workspace(4096, 3) : nullptr;
     Q.smax = smax; Q.nchk = nchk; Q.kba = kba; Q.slice_max = slice_max; Q.ns = nstg;
 
@@ -931,5 +810,5 @@ template int launch_sd_tc<22, 3>(const SdParams&, cudaStream_t, int*);
 
 }  // namespace b200trk
 
-// 1 when the most recent steepest-descent optimiser call on this process ran the tcgen05 kernel, 0 for the CUDA-core kernel
+// 1 when the most recent steepest-descent optimiser call on this process ran the tensor-core kernel, 0 for the CUDA-core kernel
 extern "C" int b200trk_sd_last_kernel(void) { return b200trk::g_sd_last_tc.load(); }

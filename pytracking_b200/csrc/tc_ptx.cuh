@@ -1,5 +1,6 @@
-// PTX wrappers shared by the tcgen05 kernels (conv_tc.cu, sd_tc.cu): mbarrier, TMA tensor loads, tcgen05.mma (kind::tf32),
-// TMEM loads, the K-major SWIZZLE_128B shared-memory descriptor and the truncation split used for 3xTF32.
+// PTX wrappers shared by the Hopper tensor-core kernels (conv_tc.cu, sd_tc.cu): mbarrier, TMA tensor loads, warpgroup MMAs
+// (wgmma.mma_async, TF32 in / FP32 accumulate in registers), the K-major SWIZZLE_128B shared-memory descriptor and the split used
+// for 3xTF32.
 #pragma once
 #include "common.cuh"
 #include <cuda.h>
@@ -17,8 +18,8 @@ __device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)_
 __device__ __forceinline__ void mbar_init(uint32_t bar, uint32_t count) {
     asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(bar), "r"(count) : "memory");
 }
-__device__ __forceinline__ void mbar_expect_tx(uint32_t bar, uint32_t bytes) {
-    asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(bar), "r"(bytes) : "memory");
+__device__ __forceinline__ void mbar_arrive(uint32_t bar) {
+    asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(bar) : "memory");
 }
 __device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity) {
     uint32_t ok = 0, spins = 0;
@@ -34,56 +35,6 @@ __device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity) {
         }
     }
 }
-__device__ __forceinline__ void tma_load_4d(uint32_t dst, const CUtensorMap* map, uint32_t bar, int c0, int c1, int c2, int c3) {
-    asm volatile("cp.async.bulk.tensor.4d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5, %6}], [%2];"
-                 ::"r"(dst), "l"((uint64_t)map), "r"(bar), "r"(c0), "r"(c1), "r"(c2), "r"(c3) : "memory");
-}
-__device__ __forceinline__ void tma_load_2d(uint32_t dst, const CUtensorMap* map, uint32_t bar, int c0, int c1) {
-    asm volatile("cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], [%2];"
-                 ::"r"(dst), "l"((uint64_t)map), "r"(bar), "r"(c0), "r"(c1) : "memory");
-}
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_commit(uint32_t bar) {
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(bar) : "memory");
-}
-// D[tmem] (+)= A[smem] * B[smem], kind::tf32, single CTA
-__device__ __forceinline__ void tc_mma_tf32(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t accumulate) {
-    asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\ttcgen05.mma.cta_group::1.kind::tf32 [%0], %1, %2, %3, p;\n\t}"
-                 ::"r"(tmem_d), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate) : "memory");
-}
-// K-major, SWIZZLE_128B canonical layout: rows of 128 B, 8-row swizzle atoms 1024 B apart (SBO), descriptor version 1
-__device__ __forceinline__ uint64_t make_smem_desc(uint32_t saddr) {
-    uint64_t d = 0;
-    d |= (uint64_t)((saddr & 0x3FFFFu) >> 4);
-    d |= (uint64_t)1 << 16;                 // leading byte offset (unused for swizzled K-major)
-    d |= (uint64_t)(1024 >> 4) << 32;       // stride byte offset
-    d |= (uint64_t)1 << 46;                 // version
-    d |= (uint64_t)2 << 61;                 // SWIZZLE_128B
-    return d;
-}
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, uint32_t (&v)[32]) {
-    asm volatile("tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-                 "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-                 "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-                 : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]),
-                   "=r"(v[8]), "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15]),
-                   "=r"(v[16]), "=r"(v[17]), "=r"(v[18]), "=r"(v[19]), "=r"(v[20]), "=r"(v[21]), "=r"(v[22]), "=r"(v[23]),
-                   "=r"(v[24]), "=r"(v[25]), "=r"(v[26]), "=r"(v[27]), "=r"(v[28]), "=r"(v[29]), "=r"(v[30]), "=r"(v[31])
-                 : "r"(taddr) : "memory");
-    asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_ld8(uint32_t taddr, uint32_t (&v)[8]) {
-    asm volatile("tcgen05.ld.sync.aligned.32x32b.x8.b32 {%0, %1, %2, %3, %4, %5, %6, %7}, [%8];"
-                 : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7])
-                 : "r"(taddr) : "memory");
-    asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_st16(uint32_t taddr, const uint32_t (&v)[16]) {
-    asm volatile("tcgen05.st.sync.aligned.32x32b.x16.b32 [%0], {%1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16};"
-                 ::"r"(taddr), "r"(v[0]), "r"(v[1]), "r"(v[2]), "r"(v[3]), "r"(v[4]), "r"(v[5]), "r"(v[6]), "r"(v[7]),
-                   "r"(v[8]), "r"(v[9]), "r"(v[10]), "r"(v[11]), "r"(v[12]), "r"(v[13]), "r"(v[14]), "r"(v[15]) : "memory");
-}
 __device__ __forceinline__ unsigned long long gtimer() {
     unsigned long long t;
     asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));
@@ -94,23 +45,16 @@ __device__ __forceinline__ float tf32_rna(float x) {
     asm("cvt.rna.tf32.f32 %0, %1;" : "=r"(r) : "f"(x));
     return __uint_as_float(r);
 }
-__device__ __forceinline__ float4 tc_lo_trunc(const float4& x) {
-    return make_float4(x.x - __uint_as_float(__float_as_uint(x.x) & 0xffffe000u),
-                       x.y - __uint_as_float(__float_as_uint(x.y) & 0xffffe000u),
-                       x.z - __uint_as_float(__float_as_uint(x.z) & 0xffffe000u),
-                       x.w - __uint_as_float(__float_as_uint(x.w) & 0xffffe000u));
-}
+// x = hi + lo with both parts TF32-representable (round to nearest): |x - hi - lo| <= 2^-22 |x|
 __device__ __forceinline__ void split_tf32(float x, float& hi, float& lo) {
     hi = tf32_rna(x);
     lo = tf32_rna(x - hi);
 }
+__device__ __forceinline__ void split_tf32_4(const float4& x, float4& hi, float4& lo) {
+    split_tf32(x.x, hi.x, lo.x); split_tf32(x.y, hi.y, lo.y); split_tf32(x.z, hi.z, lo.z); split_tf32(x.w, hi.w, lo.w);
+}
 
-
-// ---- warp-uniform single-issue forms ------------------------------------------------------------------------------------
-// The producer and MMA warps run their loops with ALL 32 lanes converged and let `elect.sync` pick the issuing lane inside
-// the instruction wrapper: wrapping the whole loop in `if (lane == 0)` instead makes ptxas emit an ELECT / R2UR.BROADCAST /
-// BRA.U.ANY waterfall loop around every tcgen05.mma (~100 cycles each). (In a kernel whose role branches are followed by a
-// block barrier ptxas still keeps the descriptors in vector registers and pays R2UR + VOTEU per MMA; DESIGN.md section 8.)
+// ---- single-issue forms: the whole producer warp runs its loop converged and elect.sync picks the issuing lane ----------
 __device__ __forceinline__ void mbar_expect_tx_elect(uint32_t bar, uint32_t bytes) {
     asm volatile("{\n\t.reg .pred e;\n\telect.sync _|e, 0xffffffff;\n\t@e mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;\n\t}"
                  ::"r"(bar), "r"(bytes) : "memory");
@@ -133,26 +77,45 @@ __device__ __forceinline__ void tma_load_2d_elect(uint32_t dst, const CUtensorMa
                  "@e cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], [%2];\n\t}"
                  ::"r"(dst), "l"((uint64_t)map), "r"(bar), "r"(c0), "r"(c1) : "memory");
 }
-__device__ __forceinline__ void tc_commit_elect(uint32_t bar) {
-    asm volatile("{\n\t.reg .pred e;\n\telect.sync _|e, 0xffffffff;\n\t"
-                 "@e tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];\n\t}" ::"r"(bar) : "memory");
+
+// ---- warpgroup MMA (sm_90a) -------------------------------------------------------------------------------------------------
+// Shared-memory matrix descriptor of a K-major SWIZZLE_128B operand tile: rows of 128 B (32 fp32), 8-row swizzle atoms 1024 B
+// apart (stride byte offset), tile base 1024-byte aligned. One K step of 8 TF32 elements = +32 B of start address.
+__device__ __forceinline__ uint64_t wg_desc(uint32_t saddr) {
+    return (uint64_t)((saddr & 0x3FFFFu) >> 4) | ((uint64_t)1 << 16) | ((uint64_t)(1024 >> 4) << 32) | ((uint64_t)1 << 62);
+}
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
+// keeps the compiler from moving accumulator accesses across a wait
+template <int R>
+__device__ __forceinline__ void wg_reg_fence(float (&d)[R]) {
+#pragma unroll
+    for (int i = 0; i < R; ++i) asm volatile("" : "+f"(d[i])::"memory");
+}
+// D[64 x N] += A[64 x 8] * B[N x 8]^T, TF32 operands, FP32 accumulators (fragment layout of the PTX ISA: register 4j + 2h + e of
+// thread t holds row 16 (t / 32) + (t % 32) / 4 + 8h, column 8j + 2 (t % 4) + e). _ss: A and B from shared memory; _rs: A from
+// registers (a[0..3] = rows r, r + 8 at column t % 4, then the same rows at column t % 4 + 4), B from shared memory.
+__device__ __forceinline__ void wgmma_ss_n64(float (&d)[32], uint64_t adesc, uint64_t bdesc) {
+    asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, 1, 0;\n\twgmma.mma_async.sync.aligned.m64n64k8.f32.tf32.tf32 "
+                 "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, %32, %33, p, 1, 1;\n\t}"
+                 : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+                 : "l"(adesc), "l"(bdesc) : "memory");
 }
 
-// Descriptor forms for the converged issue loops: the shared-memory descriptor is passed as its LOW 32-bit word only
-// (start address >> 4 | LBO field); the constant high word (SBO = 1024 B, version 1, SWIZZLE_128B = 0x40004040) is attached
-// inside the asm, so that the per-MMA operand arithmetic is 32-bit.
-__device__ __forceinline__ uint32_t make_smem_desc_lo(uint32_t saddr) { return ((saddr & 0x3FFFFu) >> 4) | (1u << 16); }
-__device__ __forceinline__ void tc_mma_tf32_lo(uint32_t tmem_d, uint32_t adesc_lo, uint32_t bdesc_lo, uint32_t idesc, uint32_t accumulate) {
-    asm volatile("{\n\t.reg .pred p, e;\n\t.reg .b64 da, db;\n\tmov.b64 da, {%1, 0x40004040};\n\tmov.b64 db, {%2, 0x40004040};\n\t"
-                 "elect.sync _|e, 0xffffffff;\n\tsetp.ne.b32 p, %4, 0;\n\t"
-                 "@e tcgen05.mma.cta_group::1.kind::tf32 [%0], da, db, %3, p;\n\t}"
-                 ::"r"(tmem_d), "r"(adesc_lo), "r"(bdesc_lo), "r"(idesc), "r"(accumulate) : "memory");
+__device__ __forceinline__ void wgmma_ss_n128(float (&d)[64], uint64_t adesc, uint64_t bdesc) {
+    asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, 1, 0;\n\twgmma.mma_async.sync.aligned.m64n128k8.f32.tf32.tf32 "
+                 "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, %64, %65, p, 1, 1;\n\t}"
+                 : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+                 : "l"(adesc), "l"(bdesc) : "memory");
 }
-__device__ __forceinline__ void tc_mma_tf32_ts_lo(uint32_t tmem_d, uint32_t tmem_a, uint32_t bdesc_lo, uint32_t idesc, uint32_t accumulate) {
-    asm volatile("{\n\t.reg .pred p, e;\n\t.reg .b64 db;\n\tmov.b64 db, {%2, 0x40004040};\n\t"
-                 "elect.sync _|e, 0xffffffff;\n\tsetp.ne.b32 p, %4, 0;\n\t"
-                 "@e tcgen05.mma.cta_group::1.kind::tf32 [%0], [%1], db, %3, p;\n\t}"
-                 ::"r"(tmem_d), "r"(tmem_a), "r"(bdesc_lo), "r"(idesc), "r"(accumulate) : "memory");
+
+__device__ __forceinline__ void wgmma_rs_n16(float (&d)[8], const uint32_t (&a)[4], uint64_t bdesc) {
+    asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, 1, 0;\n\twgmma.mma_async.sync.aligned.m64n16k8.f32.tf32.tf32 "
+                 "{%0, %1, %2, %3, %4, %5, %6, %7}, {%8, %9, %10, %11}, %12, p, 1, 1;\n\t}"
+                 : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7])
+                 : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(bdesc) : "memory");
 }
 
 // Host: fp32 tensor map (element strides 1, zero OOB fill) of rank 2..4, SWIZZLE_128B (box[0] = 32) or no swizzle; `strides_bytes`

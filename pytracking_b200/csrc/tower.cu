@@ -2,7 +2,7 @@
 //   feats_att = attention * feat                         (attention = apply_filter(feat, filter_proj): the 1x1 correlation, filter.py:60-88)
 //   tower     = 4 x [conv3x3(C -> C) + GroupNorm(1, C) + ReLU]          (heads.py:8-15)
 //   ltrb      = exp(conv3x3(C -> 4))
-// The convolutions run on the same plan machinery as the backbone (conv_tc.cu, 3xTF32 on tcgen05; the C -> 4 layer on the fp32
+// The convolutions run on the same plan machinery as the backbone (conv_tc.cu, 3xTF32 on wgmma; the C -> 4 layer on the fp32
 // CUDA-core kernel); GroupNorm(1, C) is a per-sample normalisation over C*H*W with a per-channel affine, done in place on the NHWC
 // activation by one CTA per sample (deterministic two-pass reduction).
 #include "net.cuh"

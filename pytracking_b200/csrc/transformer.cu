@@ -4,7 +4,7 @@
 // (packed in_proj, scaling 1/sqrt(head_dim), key_padding_mask -> -inf), dropout = identity (eval).
 //
 // All token-wise linear layers (QK / V / output projections, FFN 256->2048->256, decoder K/V of the memory) run on the
-// tcgen05 3xTF32 implicit-GEMM kernel of conv_tc.cu as 1x1 convolutions over the [L*B, D] token matrix (bias, ReLU and the
+// 3xTF32 wgmma implicit-GEMM kernel of conv_tc.cu as 1x1 convolutions over the [L*B, D] token matrix (bias, ReLU and the
 // residual add fused in its epilogue); attention is an fp32 online-softmax kernel (4 lanes per query, K/V tiles staged in
 // shared memory); LayerNorm is one warp per token; the decoder's 1-token linear layers are warp-per-output GEMVs.
 #include "net.cuh"
@@ -26,7 +26,7 @@ using namespace b200trk;
 struct b200trk_transformer {
     int D = 0, H = 0, FF = 0, L = 0, B = 0, n_enc = 0, n_dec = 0, M = 0;
     b200trk_net box;                      // container for the GEMM plan: buffers, split-K workspace, SM count
-    std::vector<Op> gemms;                // tcgen05 GEMMs in execution order
+    std::vector<Op> gemms;                // tensor-core GEMMs in execution order
     struct Lin { float *w = nullptr, *b = nullptr; };
     struct LN { float *g = nullptr, *b = nullptr; };
     struct Enc { Lin qk, v, o, f1, f2; LN n1, n2; int g_qk, g_v, g_o, g_f1, g_f2; };

@@ -1,7 +1,7 @@
 // The CUDA-core kernels of transformer.cu (position add, LayerNorm, the decoder's small linear layers, multi-head attention with online
 // softmax, single-query attention; references in transformer.cu's header comment).  Plain SIMT CUDA C in a header of their own so that the
 // SAME source also compiles as host code under tests/cpu_emul/cuda_shim.h (tests/test_transformer_kernels_cpu.py).  Included by
-// transformer.cu only (the token-wise linear layers of the encoder are tcgen05 GEMMs and stay there).
+// transformer.cu only (the token-wise linear layers of the encoder are tensor-core GEMMs and stay there).
 #pragma once
 
 #ifndef B200_DYN_SMEM_F
@@ -69,8 +69,7 @@ __global__ void small_linear_kernel(const float* __restrict__ x, const float* __
 // nn.MultiheadAttention core: O[lq,b,h,:] = softmax_l(Q[lq,b,h,:] . K[l,b,h,:] / sqrt(32) + mask) V[l,b,h,:]
 // head_dim = 32. Q/K/V are token-major with leading dimensions ldq/ldk/ldv (floats per token).
 // CTA = 16 queries of one (b, h); 8 lanes per query split the keys of each 64-key tile and take them FOUR at a time: four
-// independent 32-term dot products (the single dependent FMA chain per key was the latency bound of the first version,
-// profiles/r02k_ncu_summary_all_kernels.txt), one running-maximum update per group, then the four rows of V.  Online softmax per
+// independent 32-term dot products (a single dependent FMA chain per key is latency-bound), one running-maximum update per group, then the four rows of V.  Online softmax per
 // lane, the 8 partial states of a query merged with shuffles at the end (fixed order => deterministic).
 constexpr int AT_Q = 16, AT_LPQ = 8, AT_KT = 64, AT_HD = 32;
 __global__ void __launch_bounds__(128) attention_kernel(const float* __restrict__ Q, const float* __restrict__ Kp,

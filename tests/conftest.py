@@ -27,7 +27,7 @@ def pytest_configure(config):
         torch.set_num_threads(max(1, min(16, _usable_cores())))
     except Exception:
         pass
-    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on the B200 box with -m gpu)")
+    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on an H100 with -m gpu)")
 
 
 @pytest.fixture(scope="session")

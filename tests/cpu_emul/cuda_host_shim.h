@@ -42,7 +42,7 @@ static inline void* workspace(size_t bytes, int slot = 0) {
 }
 static inline int device_sm_count() {
     const char* e = std::getenv("B200_EMUL_SMS");
-    return e ? std::atoi(e) : 148;
+    return e ? std::atoi(e) : 132;        // an H100 SXM
 }
 
 }  // namespace b200trk

@@ -10,7 +10,7 @@
 using namespace b200trk;
 
 // plain build: one OS thread per CUDA thread (ThreadSanitizer sees every hand-over; small grids).  -DB200_EMUL_COOP_FIBERS: a block = one OS
-// thread, its threads = fibers -- the launch plan of a real B200 (148 CTAs x 256 threads) at ECO's real block sizes becomes affordable.
+// thread, its threads = fibers -- the launch plan of a real H100 (132 CTAs x 256 threads) at ECO's real block sizes becomes affordable.
 #ifdef B200_EMUL_COOP_FIBERS
 #define ECO_LAUNCH cpu_emul::launch_coop
 #else

@@ -1,6 +1,6 @@
 """The bench.py JSON contract, checked on the committed lines of the last GPU runs (profiles/r02_*.json): every key the driver and
 the judge read is present with the right type, the derived numbers are self-consistent, and the reference arm mirrors the b200 arm's
-metric / unit / config."""
+metric / unit / config.  r02_bench_dump_outputs.json is the line of a run with --dump-outputs: writing the outputs must not change it."""
 import json
 import os
 
@@ -27,7 +27,7 @@ def _check_common(d):
         assert k in d["e2e"], k
 
 
-@pytest.mark.parametrize("name", ["r02_bench.json", "r02_scale_n2.json"])
+@pytest.mark.parametrize("name", ["r02_bench.json", "r02_bench_dump_outputs.json"])
 def test_b200_arm_line(name):
     d = _load(name)[-1]
     _check_common(d)
@@ -50,7 +50,7 @@ def test_b200_arm_line(name):
         assert b["kind"] in ("reference", "port") and b["unit"] == d["unit"] and b["value"] < d["value"]
 
 
-@pytest.mark.parametrize("name,arm", [("r02_bench_reference_arm.json", "r02_bench.json"), ("r02_scale_n2_reference.json", "r02_scale_n2.json")])
+@pytest.mark.parametrize("name,arm", [("r02_bench_reference_arm.json", "r02_bench.json"), ("r02_bench_reference_arm.json", "r02_bench_dump_outputs.json")])
 def test_reference_arm_line_mirrors_the_b200_arm(name, arm):
     r, d = _load(name)[-1], _load(arm)[-1]
     _check_common(r)
@@ -62,19 +62,11 @@ def test_reference_arm_line_mirrors_the_b200_arm(name, arm):
     assert b["value"] == r["value"] and b["kind"] in ("reference", "port") and b["cores"] >= r["n_gpus"]
 
 
-def test_other_configuration_lines():
-    lines = _load("r02_bench_other_configs.jsonl")
-    assert len(lines) == 3
-    for d in lines:
-        _check_common(d)
-        assert d["value"] > d["torch_cuda_baseline"]["value"] > 0 and d["cpu_baseline"]["value"] > 0
-
-
 def test_eco_rows_of_the_roofline_list():
     """bench.py appends the ECO rows (tools/eco_bench.py in a subprocess) to `rooflines[]`: without a GPU the row says so instead of
     raising; with the tool's output it carries the roofline keys."""
     import bench
-    peaks = {"hbm_gbs": 6572.2}
+    peaks = {"hbm_gbs": 3350.0}
     rows = bench.eco_rows(peaks)
     assert len(rows) == 1 and "unavailable" in rows[0]                       # no CUDA device here
     data = {"deep 15x8 x 200 x 64": {"us_median": 40.0, "us_min": 39.0, "sample_memory_bytes": 12288000, "reference_sweep_bytes": 147456000,

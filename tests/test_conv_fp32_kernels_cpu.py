@@ -3,7 +3,7 @@
 deterministic split-K path (the engine's exact-fp32 `precision=1` path), NHWC -> NCHW export and `InstanceL2Norm` -- executed ON THE CPU: the
 same source file the CUDA build compiles (per-function `cuobjdump -sass` identical before and after the kernels moved into the header),
 built as host code under tests/cpu_emul/cuda_shim.h with the launch arithmetic of csrc/conv_fp32.cu, against plain PyTorch (float64).
-With tests/test_dimp_kernels_cpu.py and tests/test_corr_kernels_cpu.py every kernel of a tracked DiMP frame except the two tcgen05 ones
+With tests/test_dimp_kernels_cpu.py and tests/test_corr_kernels_cpu.py every kernel of a tracked DiMP frame except the two wgmma ones
 (`conv_tc_kernel`, `sd_tc_kernel`) also runs in the CPU tier."""
 import ctypes as C
 import os

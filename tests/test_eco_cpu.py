@@ -4,7 +4,7 @@
     per CUDA thread, pthread barriers for bar.sync / shuffles / the grid barrier -- against the same golden vectors, over several
     decompositions (grid, block, lane groups per coefficient, resident / streamed slabs), and once under ThreadSanitizer (a missing
     barrier in the kernel is a data race between the emulating threads);
-  * the launch plan at ECO's real block sizes (shared memory within the B200 limit, residency as DESIGN 4.9 states);
+  * the launch plan at ECO's real block sizes (shared memory within the 227 KB a block may use, every slab resident where it fits);
   * the plug-in seam: FilterOptim.run falls through to the reference for CPU tensors.
 """
 import ctypes as C
@@ -127,7 +127,7 @@ def test_emulated_kernel_under_thread_sanitizer(gold, tmp_path):
 
 def test_launch_plan_at_eco_block_sizes(emul):
     """ECO default (parameter/eco/default.py): memory 200, deep block 64 channels on ~15x8 coefficients, shallow block 16 channels on
-    ~63x32; 148 SMs, 256 threads."""
+    ~63x32; 148 SMs and the H100's 132, 256 threads."""
     out = (C.c_longlong * 8)()
     emul.eco_emul_plan(15, 8, 200, 64, 5, 148, 256, out)
     grid, G, CPL, GPP, res, npx_max, smem, ws = list(out)
@@ -136,6 +136,15 @@ def test_launch_plan_at_eco_block_sizes(emul):
     grid, G, CPL, GPP, res, npx_max, smem, ws = list(out)
     assert (grid, G, CPL, GPP, npx_max) == (148, 16, 1, 1, 14) and res == 8 and smem <= 227 * 1024  # 8 of <= 14 slabs resident
     emul.eco_emul_plan(31, 16, 250, 128, 5, 148, 256, out)                                          # a slab larger than shared memory
+    assert out[4] == 0 and out[6] <= 227 * 1024
+    # the launch an H100 makes (132 SMs): the deep block as above, the shallow block with <= 16 coefficients per CTA, 8 of them resident
+    emul.eco_emul_plan(15, 8, 200, 64, 5, 132, 256, out)
+    grid, G, CPL, GPP, res, npx_max, smem, ws = list(out)
+    assert (grid, G, CPL, GPP, res, npx_max) == (120, 32, 2, 8, 1, 1) and smem <= 227 * 1024
+    emul.eco_emul_plan(63, 32, 200, 16, 5, 132, 256, out)
+    grid, G, CPL, GPP, res, npx_max, smem, ws = list(out)
+    assert (grid, G, CPL, GPP, npx_max) == (132, 16, 1, 1, 16) and res == 8 and smem <= 227 * 1024
+    emul.eco_emul_plan(31, 16, 250, 128, 5, 132, 256, out)
     assert out[4] == 0 and out[6] <= 227 * 1024
 
 
@@ -334,7 +343,7 @@ def test_joint_launch_plan_at_eco_block_sizes(emul):
         assert (227 * 1024 - 1024 - fixed) // slab >= 1                # at least one coefficient's slab resident per CTA
 
 
-# The WHOLE launch of a B200 (148 CTAs x 256 threads) at ECO's default sizes runs in tests/test_eco_gpu_file_on_cpu.py: the `-m gpu` test file
+# The WHOLE launch of an H100 (132 CTAs x 256 threads) at ECO's default sizes runs in tests/test_eco_gpu_file_on_cpu.py: the `-m gpu` test file
 # itself against the launchers' host code and these kernel sources.
 
 

@@ -593,7 +593,7 @@ def test_small_stage2_ops(ops):
 @pytest.mark.parametrize("mode,n,c,h,it", [("dimp", 40, 128, 18, 3), ("prdimp", 9, 256, 22, 3), ("l2", 6, 128, 22, 3), ("hinge_relu", 7, 128, 18, 3),
                                            ("hinge_bent", 35, 256, 18, 2), ("dimp", 1, 512, 18, 2)])
 def test_sd_tensor_core_kernel_matches_cuda_core_kernel(ops, monkeypatch, mode, n, c, h, it):
-    """The tcgen05 optimiser kernel (sd_tc.cu, B200TRK_SD_TC=1) and the CUDA-core kernel (sd_optimizer.cu, =0) implement the same four
+    """The tensor-core optimiser kernel (sd_tc.cu, B200TRK_SD_TC=1) and the CUDA-core kernel (sd_optimizer.cu, =0) implement the same four
     reference optimisers; the golden cases with C % 128 != 0 only reach the latter, so every mode is also compared kernel against kernel."""
     from pytracking_b200 import _lib
     g = torch.Generator().manual_seed(100 + n)
@@ -661,7 +661,7 @@ def _rel_elem(a, b, floor=1e-3):
 
 
 def test_prdimp_sd_full_size_on_tensor_core_kernel_vs_oracle(ops, monkeypatch):
-    """PrDiMP-50 at BASELINE configs[2] size (n = 50, C = 512, 22x22 features, 23x23 scores, 10 Newton iterations) on the tcgen05
+    """PrDiMP-50 at BASELINE configs[2] size (n = 50, C = 512, 22x22 features, 23x23 scores, 10 Newton iterations) on the tensor-core
     kernel against the CPU oracle (round 1 only compared the two CUDA kernels with each other at this size)."""
     from oracle import dimp_oracle as O
     monkeypatch.setenv("B200TRK_SD_TC", "1")

@@ -1,15 +1,23 @@
 """-m gpu parity tests of the IoUNet row (SURVEY.md 8(f).1): the IoU feature branch of the network plan, `predict_iou` with its
-analytic box gradient, and the on-device refinement loops -- against the UNMODIFIED reference modules (baseline/_ref): PyTorch-CUDA
-(cuDNN / cuBLAS, TF32 off, autograd) with the library's PrRoIPool at the reference's `_prroi_pooling` seam, and PyTorch-CPU with the
-oracle's independent PrRoIPool restatement."""
+analytic box gradient, and the on-device refinement loops -- against outputs of the UNMODIFIED reference modules on the same seeded
+weights and inputs (PyTorch-CPU autograd, the oracle's PrRoIPool restatement; tests/golden/iou_tomp_ref.npz, recorded by
+oracle/gen_iou_tomp_golden.py).  The plug-in seam test runs the reference's own autograd code above the engine and needs a reference
+checkout."""
 import numpy as np
 import pytest
 import torch
 
+from ref_weights import GOLDEN, iou_inputs, iou_state_dict
+
 pytestmark = pytest.mark.gpu
 
 
-def _setup():
+def _gold():
+    return np.load(GOLDEN)
+
+
+def _ref_net():
+    """The unmodified reference DiMP-50 network with the golden's weights (for the plug-in seam test only)."""
     from baseline import ref_env
     if not ref_env.reference_available():
         pytest.skip("reference tree not staged (baseline/_ref)")
@@ -19,16 +27,8 @@ def _setup():
     torch.backends.cuda.matmul.allow_tf32 = False
     from baseline import ref_tracker
     net = ref_tracker.build_dimp_net("resnet50", seed=0)
-    # non-trivial BN statistics in the IoUNet (the constructor leaves running_mean 0 / running_var 1)
-    g = torch.Generator().manual_seed(5)
-    for m in net.bb_regressor.modules():
-        if isinstance(m, torch.nn.BatchNorm2d):
-            m.running_mean.copy_(0.05 * torch.randn(m.running_mean.shape, generator=g))
-            m.running_var.copy_(0.7 + 0.6 * torch.rand(m.running_var.shape, generator=g))
-            m.bias.data.copy_(0.05 * torch.randn(m.bias.shape, generator=g))
-    with torch.no_grad():
-        net.bb_regressor.iou_predictor.weight.mul_(20.0)      # box gradients of O(1e-2): the refinement loops move boxes by pixels
-    return net
+    net.load_state_dict(iou_state_dict(_gold()), strict=False)
+    return net.eval()
 
 
 def _rel(a, b):
@@ -42,40 +42,65 @@ def _rel_elem(a, b, floor):
     return float(((a - b).abs() / b.abs().clamp(min=floor * b.abs().max())).max())
 
 
+def _sampled_rel(mine, gold, name, floor=None):
+    """Relative error of `mine` at the golden's sampled indices: against the full reference maximum, or element-wise with the
+    denominator floored at `floor` x that maximum."""
+    a = mine.detach().double().cpu().reshape(-1)[torch.from_numpy(gold[name + "_idx"])]
+    b = torch.from_numpy(gold[name]).double()
+    amax = float(gold[name + "_amax"])
+    if floor is None:
+        return float((a - b).abs().max() / amax)
+    return float(((a - b).abs() / b.abs().clamp(min=floor * amax)).max())
+
+
 def test_iou_feature_branch_matches_reference_get_iou_feat():
-    net = _setup()
+    gold = _gold()
+    sd = iou_state_dict(gold)
     from pytracking_b200 import synth
     from pytracking_b200.engine import BackboneEngine
     im = synth.make_crop(3, 2, 288)
-    eng = BackboneEngine(net.state_dict(), arch="resnet50", max_batch=2, crop_size=288)
-    eng.attach_iou_head(net.state_dict())
+    eng = BackboneEngine(sd, arch="resnet50", max_batch=2, crop_size=288)
+    eng.attach_iou_head(sd)
     out = eng.forward(im.cuda(), want=("layer2", "layer3", "iou3", "iou4"))
     again = eng.iou_features(2)                                   # the branch alone, from the arena
     assert torch.equal(again[0], out["iou3"]) and torch.equal(again[1], out["iou4"])
-    with torch.no_grad():
-        x = (im / 255 - torch.tensor([0.485, 0.456, 0.406]).view(1, 3, 1, 1)) / torch.tensor([0.229, 0.224, 0.225]).view(1, 3, 1, 1)
-        bf = net.extract_backbone_features(x)                      # CPU reference
-        c3, c4 = net.bb_regressor.get_iou_feat([bf["layer2"], bf["layer3"]])
-        netc = net.cuda()
-        bfc = netc.extract_backbone_features(x.cuda())             # PyTorch-CUDA reference
-        c3c, c4c = netc.bb_regressor.get_iou_feat([bfc["layer2"], bfc["layer3"]])
-    for mine, ref_cpu, ref_cuda in ((out["iou3"], c3, c3c), (out["iou4"], c4, c4c)):
-        assert _rel(mine, ref_cpu) < 1e-4 and _rel(mine, ref_cuda) < 1e-4, (_rel(mine, ref_cpu), _rel(mine, ref_cuda))
+    for mine, name in ((out["iou3"], "feat_c3"), (out["iou4"], "feat_c4")):
+        assert _sampled_rel(mine, gold, name) < 1e-4, (name, _sampled_rel(mine, gold, name))
         # element-wise: entries above 1 % of the map's maximum to 2e-3 (two more 3x3 layers after layer2 / layer3)
-        assert _rel_elem(mine, ref_cpu, 1e-2) < 2e-3, _rel_elem(mine, ref_cpu, 1e-2)
+        assert _sampled_rel(mine, gold, name, 1e-2) < 2e-3, (name, _sampled_rel(mine, gold, name, 1e-2))
     eng.close()
-    net.cpu()
 
 
-def _inputs(net, seed, R):
-    g = torch.Generator().manual_seed(seed)
-    f3 = torch.relu(torch.randn(1, 256, 36, 36, generator=g))
-    f4 = torch.relu(torch.randn(1, 256, 18, 18, generator=g))
-    mod = [torch.randn(1, 256, 1, 1, generator=g).abs(), torch.randn(1, 256, 1, 1, generator=g).abs()]
-    c = torch.tensor([120.0, 130.0]) + 30 * (torch.rand(R, 2, generator=g) - 0.5)
-    sz = torch.tensor([70.0, 55.0]) * (0.6 + 0.8 * torch.rand(R, 2, generator=g))
-    boxes = torch.cat([c - sz / 2, sz], 1).reshape(1, R, 4)
-    return mod, [f3, f4], boxes
+def test_predict_iou_and_box_gradient_match_reference_autograd():
+    gold = _gold()
+    from pytracking_b200.iou import IoUPredictor
+    pred = IoUPredictor(iou_state_dict(gold))
+    for seed, R in ((0, 10), (1, 1), (2, 16)):
+        mod, feat, boxes = iou_inputs(seed, R)
+        iou, grad = pred.predict_iou([m.cuda() for m in mod], [f.cuda() for f in feat], boxes.cuda(), return_grad=True)
+        ref_i, ref_g = torch.from_numpy(gold["piou_%d_iou" % seed]), torch.from_numpy(gold["piou_%d_grad" % seed])
+        assert _rel(iou, ref_i) < 1e-4, (seed, _rel(iou, ref_i))
+        assert _rel(grad, ref_g) < 1e-4, (seed, _rel(grad, ref_g))
+        assert _rel_elem(iou, ref_i, 1e-3) < 1e-3
+    pred.close()
+
+
+@pytest.mark.parametrize("relative", [False, True])
+def test_refinement_loop_matches_reference_optimize_boxes(relative):
+    gold = _gold()
+    from pytracking_b200.iou import IoUPredictor
+    pred = IoUPredictor(iou_state_dict(gold))
+    mod, feat, boxes = iou_inputs(7, 10)
+    iters, step = (10, 2.5e-3) if relative else (5, 1.0)
+    ref_boxes = torch.from_numpy(gold["refine_%d_%d_boxes" % (iters, relative)])
+    ref_iou = torch.from_numpy(gold["refine_%d_%d_iou" % (iters, relative)])
+    b, iou = pred.refine([m.cuda() for m in mod], [f.cuda() for f in feat], boxes.cuda(), iters, step, 1, relative)
+    assert _rel(b, ref_boxes) < 1e-4, _rel(b, ref_boxes)
+    assert float((b.cpu() - ref_boxes).abs().max()) < 2e-2            # pixels, after 5 / 10 ascent steps of O(1..10) px each
+    assert _rel(iou, ref_iou) < 1e-3, _rel(iou, ref_iou)
+    moved = float((ref_boxes - boxes.reshape(-1, 4)).abs().max())
+    assert moved > 0.5, moved                                           # the loop really moved the boxes
+    pred.close()
 
 
 def _ref_iou_and_grad(net, mod, feat, boxes, device):
@@ -86,63 +111,10 @@ def _ref_iou_and_grad(net, mod, feat, boxes, device):
     return iou.detach().cpu(), bb.grad.detach().cpu()
 
 
-def test_predict_iou_and_box_gradient_match_reference_autograd():
-    net = _setup()
-    from pytracking_b200 import plugin
-    from pytracking_b200.iou import IoUPredictor
-    pred = IoUPredictor(net.state_dict())
-    for seed, R in ((0, 10), (1, 1), (2, 16)):
-        mod, feat, boxes = _inputs(net, seed, R)
-        iou, grad = pred.predict_iou([m.cuda() for m in mod], [f.cuda() for f in feat], boxes.cuda(), return_grad=True)
-        i_cpu, g_cpu = _ref_iou_and_grad(net, mod, feat, boxes, "cpu")          # oracle PrRoIPool (CPU restatement), torch autograd
-        # reference autograd on CUDA: the reference's own predict_iou stays, only the native PrRoIPool comes from the library
-        plugin.install(skip=("predict_iou",))
-        try:
-            i_cuda, g_cuda = _ref_iou_and_grad(net, mod, feat, boxes, "cuda")
-        finally:
-            plugin.uninstall()
-            net.cpu()
-        for ref_i, ref_g, tag in ((i_cpu, g_cpu, "cpu"), (i_cuda, g_cuda, "cuda")):
-            assert _rel(iou, ref_i) < 1e-4, (tag, seed, _rel(iou, ref_i))
-            assert _rel(grad, ref_g) < 1e-4, (tag, seed, _rel(grad, ref_g))
-            assert _rel_elem(iou, ref_i, 1e-3) < 1e-3
-    pred.close()
-
-
-@pytest.mark.parametrize("relative", [False, True])
-def test_refinement_loop_matches_reference_optimize_boxes(relative):
-    net = _setup()
-    from pytracking.tracker.dimp.dimp import DiMP
-    from pytracking.utils import TrackerParams
-    from pytracking.libs import TensorList
-    from pytracking_b200.iou import IoUPredictor
-    pred = IoUPredictor(net.state_dict())
-    mod, feat, boxes = _inputs(net, 7, 10)
-    p = TrackerParams()
-    p.device = "cpu"
-    p.box_refinement_iter = 10 if relative else 5
-    p.box_refinement_step_length = 2.5e-3 if relative else 1
-    p.box_refinement_step_decay = 1
-    p.box_refinement_space = "relative" if relative else "default"
-    trk = DiMP.__new__(DiMP)
-    trk.params = p
-    trk.net = type("N", (), {"bb_regressor": net.bb_regressor})()
-    trk.iou_modulation = TensorList(mod)
-    ref_boxes, ref_iou = trk.optimize_boxes(TensorList(feat), boxes.reshape(-1, 4).clone())        # CPU reference loop (autograd)
-    b, iou = pred.refine([m.cuda() for m in mod], [f.cuda() for f in feat], boxes.cuda(), p.box_refinement_iter,
-                         p.box_refinement_step_length, p.box_refinement_step_decay, relative)
-    assert _rel(b, ref_boxes) < 1e-4, _rel(b, ref_boxes)
-    assert float((b.cpu() - ref_boxes).abs().max()) < 2e-2            # pixels, after 5 / 10 ascent steps of O(1..10) px each
-    assert _rel(iou, ref_iou) < 1e-3, _rel(iou, ref_iou)
-    moved = float((ref_boxes - boxes.reshape(-1, 4)).abs().max())
-    assert moved > 0.5, moved                                           # the loop really moved the boxes
-    pred.close()
-
-
 def test_plugin_predict_iou_seam_keeps_the_trackers_autograd_code_working():
-    net = _setup()
+    net = _ref_net()
     from pytracking_b200 import plugin
-    mod, feat, boxes = _inputs(net, 11, 10)
+    mod, feat, boxes = iou_inputs(11, 10)
     i_cpu, g_cpu = _ref_iou_and_grad(net, mod, feat, boxes, "cpu")
     plugin.install()
     plugin.stats.clear()

@@ -1,9 +1,13 @@
 """-m gpu parity tests of the ToMP row (SURVEY.md 8(a) T1) beyond `Transformer.forward` (tests/test_gpu_parity.py): the head feature
-extractor on the network plan, the `DenseBoxRegressor` tower on the engine, and the UNMODIFIED reference ToMP-101 tracker
-(pytracking/tracker/tomp/tomp.py, baseline/_ref) above the engine against the same tracker on stock PyTorch-CUDA (TF32 off)."""
+extractor on the network plan, the `DenseBoxRegressor` tower and the token assembly on the engine against outputs of the UNMODIFIED
+reference modules on the same seeded weights and inputs (tests/golden/iou_tomp_ref.npz, oracle/gen_iou_tomp_golden.py), and the
+unmodified reference ToMP-101 tracker (pytracking/tracker/tomp/tomp.py) above the engine against the same tracker on stock PyTorch-CUDA
+(TF32 off; needs a reference checkout)."""
 import numpy as np
 import pytest
 import torch
+
+from ref_weights import GOLDEN, token_inputs, token_state_dict, tower_inputs, tower_state_dict
 
 pytestmark = pytest.mark.gpu
 
@@ -24,29 +28,17 @@ def _rel(a, b):
 
 
 def test_box_regression_tower_matches_reference_module():
-    _ref()
-    import ltr.models.transformer.heads as heads
     from pytracking_b200.transformer_engine import BoxTower
-    torch.manual_seed(3)
-    m = heads.DenseBoxRegressor(num_channels=256).eval()
-    g = torch.Generator().manual_seed(4)
-    with torch.no_grad():
-        for p in m.parameters():                       # non-trivial GroupNorm affines / biases
-            if p.dim() == 1:
-                p.copy_(0.5 + torch.rand(p.shape, generator=g) if p.numel() == 256 and p.mean() > 0.5 else 0.1 * torch.randn(p.shape, generator=g))
-        m.bbreg_layer.weight.mul_(0.3)
-    feat = torch.randn(1, 1, 256, 18, 18, generator=g) * 0.3
-    filt = torch.randn(1, 256, 1, 1, generator=g) * 0.2
-    with torch.no_grad():
-        ref_cpu = m(feat, filt)                                               # [1,1,4,18,18]
-        mc = m.cuda()
-        ref_cuda = mc(feat.cuda(), filt.cuda())
-        fp = mc.linear(filt.cuda().reshape(-1, 256)).reshape(1, 256, 1, 1)
-        att = (feat.cuda()[0] * fp).sum(1)                                     # the 1x1 correlation
-    tw = BoxTower(m.state_dict(), 18, 18, max_batch=2)
+    gold = np.load(GOLDEN)
+    sd = tower_state_dict(gold)
+    feat, filt = tower_inputs()
+    ref = torch.from_numpy(gold["tower_out"])                                  # DenseBoxRegressor.forward: [1, 4, 18, 18]
+    fp = (filt.reshape(1, 256) @ sd["linear.weight"].t() + sd["linear.bias"]).reshape(1, 256, 1, 1).cuda()
+    att = (feat.cuda()[0] * fp).sum(1)                                          # the 1x1 correlation
+    tw = BoxTower(sd, 18, 18, max_batch=2)
     out = tw.forward(feat.cuda()[0], att)
     assert out.shape == (1, 4, 18, 18)
-    assert _rel(out, ref_cpu[0]) < 1e-4 and _rel(out, ref_cuda[0]) < 1e-4, (_rel(out, ref_cpu[0]), _rel(out, ref_cuda[0]))
+    assert _rel(out, ref) < 1e-4, _rel(out, ref)
     assert abs(tw.flops / 2 / 1e6 - (4 * 191.1 + 191.1 * 4 / 256)) < 2.0      # 9 * 256 * 256 * 324 = 191.1 MMAC per 256 -> 256 layer at 18x18
     two = tw.forward(torch.cat([feat.cuda()[0], feat.cuda()[0]]), torch.cat([att, att]))
     # the two samples of one launch are bitwise identical; a batch-1 launch may pick another split-K factor (different summation order)
@@ -80,39 +72,19 @@ def test_reference_tomp_tracker_above_engine():
 
 
 def test_token_assembly_matches_reference_filter_predictor():
-    """`b200trk_tomp_tokens` against the reference's own token construction (filter_predictor.py:92-135), intercepted at the
-    transformer call, for 2 training frames + 1 test frame; with and without the test-frame embedding."""
-    _ref()
-    import ltr.models.transformer.filter_predictor as fp
+    """`b200trk_tomp_tokens` against the tokens the reference's FilterPredictor hands to its transformer (filter_predictor.py:92-135)
+    for 2 training frames + 1 test frame, with and without the test-frame embedding."""
     from pytracking_b200.transformer_engine import TokenBuilder
-    for use_test in (False, True):
-        captured = {}
-
-        class FakeTransformer(torch.nn.Module):
-            d_model = 256
-
-            def forward(self, feat, mask=None, query_embed=None, pos_embed=None):
-                captured["feat"], captured["mask"], captured["pos"] = feat.clone(), mask, pos_embed
-                return torch.zeros(1, 1, feat.shape[1], 256), torch.zeros_like(feat)
-        torch.manual_seed(7)
-        m = fp.FilterPredictor(FakeTransformer(), feature_sz=18, use_test_frame_encoding=use_test).eval()
-        g = torch.Generator().manual_seed(8)
-        with torch.no_grad():
-            for mod in m.box_encoding:
-                if isinstance(mod, torch.nn.BatchNorm1d):
-                    mod.running_mean.copy_(0.1 * torch.randn(mod.running_mean.shape, generator=g))
-                    mod.running_var.copy_(0.6 + 0.8 * torch.rand(mod.running_var.shape, generator=g))
-                    mod.weight.copy_(0.8 + 0.4 * torch.rand(mod.weight.shape, generator=g))
-                    mod.bias.copy_(0.1 * torch.randn(mod.bias.shape, generator=g))
-        train_feat = torch.randn(2, 1, 256, 18, 18, generator=g)
-        test_feat = torch.randn(1, 1, 256, 18, 18, generator=g)
-        label = torch.rand(2, 1, 18, 18, generator=g)
-        ltrb = torch.rand(2, 1, 4, 18, 18, generator=g)
-        with torch.no_grad():
-            m.predict_cls_bbreg_filters_parallel(train_feat, test_feat, label, 1, ltrb)
-        ref = captured["feat"]                                                      # [972, 2, 256]
-        tb = TokenBuilder(m.state_dict())
-        out = tb.build(train_feat[:, 0].cuda(), test_feat[:, 0].cuda(), label[:, 0].cuda(), ltrb[:, 0].cuda(), B=2, use_test_token=use_test)
-        assert out.shape == ref.shape
-        assert _rel(out, ref) < 1e-5, _rel(out, ref)
-        assert captured["mask"].shape == (2, 972) and int(captured["mask"][1].sum()) == 324 and int(captured["mask"][0].sum()) == 0
+    gold = np.load(GOLDEN)
+    train_feat, test_feat, label, ltrb = token_inputs()
+    for use_test in (0, 1):
+        sd = token_state_dict(gold, use_test)
+        tb = TokenBuilder(sd)
+        out = tb.build(train_feat[:, 0].cuda(), test_feat[:, 0].cuda(), label[:, 0].cuda(), ltrb[:, 0].cuda(), B=2, use_test_token=bool(use_test))
+        assert tuple(out.shape) == tuple(gold["tok%d_feat_shape" % use_test])                 # [972, 2, 256]
+        name = "tok%d_feat" % use_test
+        a = out.detach().double().cpu().reshape(-1)[torch.from_numpy(gold[name + "_idx"])]
+        err = float((a - torch.from_numpy(gold[name]).double()).abs().max() / float(gold[name + "_amax"]))
+        assert err < 1e-5, (use_test, err)
+        mask = gold["tok%d_mask" % use_test]
+        assert mask.shape == (2, 972) and int(mask[1].sum()) == 324 and int(mask[0].sum()) == 0

@@ -17,6 +17,32 @@ OVERRIDES = {
 }
 
 
+def random_localize_cases(n=400):
+    """Seeded localisation problems for the localisation kernel (score maps with a few peaks and exact ties, thresholds, geometry):
+    yields (trial, params overrides, scores [S,19,19], target_sz, sample_scales, sample_pos, pos).  The reference's answers to the
+    same problems are tests/golden/dimp_localize_random.npz (oracle/gen_host_logic_golden.py)."""
+    import torch
+    g = torch.Generator().manual_seed(0)
+    for trial in range(n):
+        S = 1 + trial % 3
+        kw = dict(advanced_localization=trial % 10 != 9, target_not_found_threshold=0.2,
+                  uncertain_threshold=0.25 if trial % 4 == 0 else -float("inf"),
+                  hard_sample_threshold=0.3 if trial % 5 == 0 else -float("inf"), distractor_threshold=0.8, hard_negative_threshold=0.5,
+                  dispalcement_scale=0.3 + 0.5 * (trial % 2))
+        scores = 0.1 * torch.rand(S, 19, 19, generator=g)
+        for s in range(S):
+            for _ in range(1 + trial % 3):               # a few peaks of comparable height
+                r, c = [int(v) for v in torch.randint(0, 19, (2,), generator=g)]
+                scores[s, r, c] = 0.15 + 0.6 * float(torch.rand(1, generator=g))
+        if trial % 7 == 0:                               # exact ties: the arg-max order must follow dcf.max2d
+            scores[0, 3, 11] = scores[0, 12, 4] = scores.max() + 0.1
+        target_sz = torch.Tensor([60, 80]) * (0.5 + float(torch.rand(1, generator=g)))
+        sample_scales = 1.0 + 0.5 * torch.rand(S, generator=g)
+        sample_pos = torch.Tensor([[240, 320]]).repeat(S, 1) + torch.rand(S, 2, generator=g)
+        pos = sample_pos[0] + 40 * (torch.rand(2, generator=g) - 0.5)
+        yield trial, kw, scores, target_sz, sample_scales, sample_pos, pos
+
+
 def _loc(d, t):
     loc = _lib.LocResult()
     loc.flag, loc.scale_ind = int(d["flag"][t]), 0

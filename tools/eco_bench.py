@@ -3,11 +3,10 @@ memory 200, CG_iter 5; deep block 64 channels on 15x8 Fourier coefficients, shal
 figures of DESIGN 4.9: bytes of sample memory per call, the reference's traffic (2 (1 + num_iter) sweeps), achieved GB/s; the first-frame
 joint optimisation; and the score computation of a tracked frame (apply_filter, sample_fs, max2d).
 
-    python tools/eco_bench.py [--json PATH]    (on a GPU box; writes gpurun_out/eco_bench.json or PATH)
+    python tools/eco_bench.py [--json PATH]    (on a GPU machine; prints the rows, or writes them to PATH)
 
 bench.py runs this file in a SUBPROCESS after its timed regions (N = 1, rank 0) and appends the rows to `rooflines[]`, so that a defect in
-these kernels -- the only ones of the library that had not been timed on a B200 when the round's GPU budget ran out -- cannot touch the
-headline measurement."""
+these kernels cannot touch the headline measurement."""
 import json
 import os
 import sys

@@ -1,6 +1,6 @@
-"""Condense `ncu -i <rep> --page raw --csv` into one line per kernel launch (profiles/*_ncu_summary.txt).
+"""Condense `ncu -i <rep> --page raw --csv` into one line per kernel launch.
 
-    ncu -i gpurun_out/r02i_all.ncu-rep --page raw --csv > /tmp/raw.csv && python tools/ncu_summary.py /tmp/raw.csv > profiles/r02_ncu_summary.txt
+    ncu -i /tmp/profile_all.ncu-rep --page raw --csv > /tmp/raw.csv && python tools/ncu_summary.py /tmp/raw.csv
 """
 import csv
 import sys

@@ -1,7 +1,7 @@
 """One launch of every kernel family of the library between cudaProfilerStart / Stop, for a single ncu pass:
 
-    ncu --set full --clock-control none --import-source on --profile-from-start off -o gpurun_out/r02_all -f python tools/profile_all.py
-    ncu --metrics gpu__time_duration.sum --clock-control none --profile-from-start off --csv --log-file gpurun_out/r02_launches.csv \
+    ncu --set full --clock-control none --import-source on --profile-from-start off -o /tmp/profile_all -f python tools/profile_all.py
+    ncu --metrics gpu__time_duration.sum --clock-control none --profile-from-start off --csv --log-file /tmp/profile_all_launches.csv \
         python tools/profile_all.py frames
 
 Default: each family once at its BASELINE size (SURVEY.md 8(d)).  `frames`: three whole tracked frames of the native tracker (the

@@ -1,4 +1,4 @@
-"""Phase trace of the tcgen05 SD kernel on the frame engine's pitched sample memory vs the dense C-ABI call."""
+"""Phase trace of the tensor-core SD kernel on the frame engine's pitched sample memory vs the dense C-ABI call."""
 import sys, os, ctypes as C
 os.environ["B200TRK_SD_TC"] = "1"; os.environ["B200TRK_SD_TRACE"] = "1"
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))

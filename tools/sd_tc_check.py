@@ -1,4 +1,4 @@
-"""tcgen05 SD sweeps (B200TRK_SD_TC=1) against the CUDA-core kernel: per-iterate errors, losses, timing, phase trace."""
+"""Tensor-core SD sweeps (B200TRK_SD_TC=1) against the CUDA-core kernel: per-iterate errors, losses, timing, phase trace."""
 import sys, os, ctypes as C
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import torch, numpy as np

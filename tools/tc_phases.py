@@ -47,13 +47,3 @@ for i, (b, info) in bufs.items():
     prev_end = end
 print("sum of spans+gaps (us):", tot)
 
-if len(sys.argv) > 2:
-    for oi in [int(x) for x in sys.argv[2].split(",")]:
-        b, info = bufs[oi]
-        tr = b[2048:2048 + 16].cpu().double()
-        base = tr[0, 0]
-        print("trace op %d (us since first slot-free): slot_free loads_issued landed split_done mma_sees mma_issued" % oi)
-        for it in range(16):
-            if tr[it, 0] == 0:
-                break
-            print("  kb %2d: " % it + " ".join("%7.2f" % (float(tr[it, k] - base) / 1e3) for k in range(6)))
