@@ -41,8 +41,8 @@ typedef struct b200trk_net b200trk_net_t;    /* opaque: folded + repacked networ
 
 int         b200trk_version(void);
 const char* b200trk_last_error(void);
-/* Debug aid: when B200TRK_SD_TRACE is set in the environment the SD optimiser kernels record 64 phase time stamps
- * (globaltimer ns) of CTA 0; this copies them to out_host[64]. */
+/* Debug aid: when B200TRK_SD_TRACE is set in the environment the SD optimiser kernels record 128 phase time stamps
+ * (globaltimer ns) of CTA 0; this copies them to out_host[128]. */
 /* 1 when the most recent steepest-descent optimiser call ran the tensor-core kernel (sd_tc.cu), 0 for the CUDA-core kernel */
 int b200trk_sd_last_kernel(void);
 int b200trk_debug_sd_trace(unsigned long long* out_host);

@@ -64,11 +64,11 @@ int device_sm_count() {
 
 }  // namespace b200trk
 
-// debug: copy the SD optimiser phase trace (64 x u64) to the host
+// debug: copy the SD optimiser phase trace (128 x u64) to the host
 extern "C" int b200trk_debug_sd_trace(unsigned long long* out_host) {
     void* p = b200trk::workspace(1024, 3);
     if (!p || !out_host) return 1;
-    return cudaMemcpy(out_host, p, 512, cudaMemcpyDeviceToHost) == cudaSuccess ? 0 : 1;
+    return cudaMemcpy(out_host, p, 1024, cudaMemcpyDeviceToHost) == cudaSuccess ? 0 : 1;
 }
 
 // debug: per-unit pipeline stamps of the tensor-core SD kernel ([16 units][16] x u64 SM clocks, CTA 0, first adjoint sweep; cleared after the read)

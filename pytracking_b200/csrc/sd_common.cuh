@@ -23,7 +23,7 @@ struct SdParams {
     float* iterates_out; float* losses_out;
     // workspace
     float* gpart; float* qpart; float* hpart; float* gnorm; float* lossr; float* lossw; unsigned* barrier;
-    unsigned long long* trace;     // optional [64] phase stamps of CTA 0 (globaltimer ns)
+    unsigned long long* trace;     // optional [128] phase stamps of CTA 0 (globaltimer ns)
 };
 
 __device__ __forceinline__ unsigned long long sd_gtimer() {
@@ -35,7 +35,7 @@ __device__ __forceinline__ unsigned long long sd_gtimer() {
     return t;
 #endif
 }
-#define SD_STAMP(k) do { if (P.trace && blockIdx.x == 0 && threadIdx.x == 0 && (k) < 64) P.trace[(k)] = sd_gtimer(); } while (0)
+#define SD_STAMP(k) do { if (P.trace && blockIdx.x == 0 && threadIdx.x == 0 && (k) < 128) P.trace[(k)] = sd_gtimer(); } while (0)
 
 __device__ __forceinline__ float lut_lerp(const float* lut, int nb, float rho) {
     // DistanceMap + 1x1 conv == piece-wise linear LUT with last-bin clamp (distance.py:33-37)

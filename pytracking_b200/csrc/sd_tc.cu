@@ -4,7 +4,7 @@
 //
 //   adjoint sweep   g[c, tap]  = sum_{i, p} X_i[c, p] * R_i[p, tap]        R_i[p, tap] = r_i[p shifted by the tap]   (A^T r)
 //       A = X_i[128 channels x 32 pixels]  (K-major straight from the [n, C, H*W] sample memory, TMA box, 128-byte swizzle)
-//       B = R_i^T[16 taps x 32 pixels]      (gathered from the residual map by the consumer threads into the stage)
+//       B = R_i^T[16 taps x 32 pixels]      (gathered from the residual map once per iteration, resident in shared memory)
 //   apply sweep     T_i[p, tap] = sum_c X_i[p, c] * F[c, tap] ;  s_i[y, x] = sum_tap T_i[(y, x) shifted by the tap, tap]   (A f)
 //       A = X_i[128 pixels x 32 channels]  (the SAME [n, C, H*W] memory: the TMA box is 32 channel rows x 128 pixels; TF32 wgmma
 //                                            wants K-major operands, so A is read transposed from shared memory into registers)
@@ -26,11 +26,13 @@
 // terms are contributed by the sample's owner (the CTA holding its first unit) only.
 //
 // Operand pipeline (per unit): warp 8 (the producer) lands the raw 128 x 32 fp32 tile in one of up to 8 shared-memory stages with
-// TMA; warps 0-7 (two consumer warpgroups, rows 0-63 / 64-127 of the tile) read their A fragments into registers, split them, and
-// issue 4 K steps x 3 products as register-A wgmmas against the 16-row B operand in shared memory. The apply sweep frees a stage
-// as soon as its fragments are in registers; the adjoint sweep also stages the unit's B tile there and frees it when the MMAs have
-// retired. The producer also issues the first units of the NEXT sweep while the CTAs sit in the grid barrier. All 288 threads
-// run the element-wise phases between the sweeps.
+// TMA; warps 0-7 (two consumer warpgroups, rows 0-63 / 64-127 of the tile) read their A fragments into registers, split them, free
+// the stage and issue 4 K steps x 3 products as register-A wgmmas against the 16-row B operand in shared memory. Two register sets
+// of fragments alternate: unit i+1 is loaded and split while unit i's MMAs are in flight, and the consumers only drain the MMAs
+// (wait_group 0) where the accumulators are read (end of a gradient chunk / an apply segment). The B tiles of both sweeps live in
+// one shared-memory region: R^T of every (sample, pixel block) pair of the CTA's adjoint range, built by all threads right after
+// the residual, then F^T of all channel blocks, built after the gradient exchange. The producer also issues the first units of
+// the NEXT sweep while the CTAs sit in the grid barrier. All 288 threads run the element-wise phases between the sweeps.
 #include "tc_ptx.cuh"
 #include "sd_common.cuh"
 #include <atomic>
@@ -43,8 +45,7 @@ constexpr int STC_CT = 256;                 // consumer threads (warps 0-7: two 
 constexpr int STC_THREADS = STC_CT + 32;    // + warp 8, the TMA producer
 constexpr int STC_NS_MAX = 8;               // shared-memory stages (runtime count Q.ns)
 constexpr int STC_NS_MIN = 4;
-constexpr int STC_A_BYTES = 16384;          // 128 rows x 128 B
-constexpr int STC_STAGE_BYTES = 20480;      // A raw | B_hi (2 KB) | B_lo (2 KB)
+constexpr int STC_STAGE_BYTES = 16384;      // raw A tile: 128 rows x 128 B
 constexpr int STC_MAXCH = 4;                // 128-channel chunks (C <= 512)
 constexpr int STC_TT_PITCH = 132;
 constexpr int STC_MAXG = 160;                // CTAs (= SMs) the partition tables are sized for
@@ -57,6 +58,7 @@ struct SdTcParams {
     float* gpart; float* gfinal; float* gnpart; float* qslots; float* hpart; float* lossr; float* lossw;
     unsigned* barrier;
     int smax, nchk, kba, slice_max, ns;
+    int nbt;                // 4 KB B tiles of the shared region: max(kba, adjoint pairs of the longest range)
 };
 
 __device__ __forceinline__ int part_lo(long long U, int G, int b) { return (int)((U * (long long)b) / G); }
@@ -107,8 +109,8 @@ __global__ void __launch_bounds__(STC_THREADS, 1) sd_tc_kernel(const __grid_cons
     uint8_t* base = stc_raw + ((1024u - (smem_u32(stc_raw) & 1023u)) & 1023u);
     const uint32_t base_u32 = smem_u32(base);
     const int NS = Q.ns;
-    uint8_t* ftb = base + NS * STC_STAGE_BYTES;                 // F^T: [kba][hi 2 KB | lo 2 KB]
-    float* Tt = reinterpret_cast<float*>(ftb + (size_t)kba * 4096);   // [16][STC_TT_PITCH] apply-epilogue staging
+    uint8_t* ftb = base + NS * STC_STAGE_BYTES;                 // B tiles [nbt][hi 2 KB | lo 2 KB]: R^T (adjoint) or F^T (apply)
+    float* Tt = reinterpret_cast<float*>(ftb + (size_t)Q.nbt * 4096);   // [16][STC_TT_PITCH] apply-epilogue staging
     float4* wsl = reinterpret_cast<float4*>(Tt + 16 * STC_TT_PITCH);  // filter slice owned by this CTA
     float4* gsl = wsl + Q.slice_max;                                  // gradient slice
     float* sS = reinterpret_cast<float*>(gsl + Q.slice_max);          // [smax][NPOS] scores
@@ -264,8 +266,34 @@ __global__ void __launch_bounds__(STC_THREADS, 1) sd_tc_kernel(const __grid_cons
         __syncthreads();
     };
 
+    // R^T (hi | lo) of every (sample, pixel block) pair of this CTA's adjoint range, from the mapped residuals. The range is
+    // contiguous in (chunk, sample, pixel block) order, so unit t_lo + i uses pair slot i mod (n KBT): min(range, n KBT) slots.
+    auto build_rt = [&]() {
+        const int per_chunk = n * KBT;
+        const int np = min(t_hi - t_lo, per_chunk);
+        for (int sl = warp; sl < np; sl += NTH / 32) {                // one warp per slot, lane = pixel of the block
+            const int r = (t_lo + sl) % per_chunk, smp = r / KBT, kb = r - smp * KBT;
+            int j = 0;
+            for (int jj = 1; jj < ns; ++jj) j = (s_state[jj] == smp) ? jj : j;
+            const int px = kb * 32 + lane, iy = px / FS, ix = px - iy * FS;
+            const float* src = sT + j * NPOS;
+            uint8_t* t = ftb + (size_t)sl * 4096;
+#pragma unroll
+            for (int tap = 0; tap < 16; ++tap) {
+                const int oy = iy - (tap >> 2) + 2, ox = ix - (tap & 3) + 2;
+                const float v = (px < NPX && oy >= 0 && oy < OS && ox >= 0 && ox < OS) ? src[oy * OS + ox] : 0.f;
+                float h, l;
+                split_tf32(v, h, l);
+                *reinterpret_cast<float*>(t + sw128(tap, lane)) = h;
+                *reinterpret_cast<float*>(t + 2048 + sw128(tap, lane)) = l;
+            }
+        }
+        asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
+        __syncthreads();
+    };
+
     // per-unit pipeline stamps (SM clock) of CTA 0 during the first adjoint sweep: utr[unit][16]
-    // 0 slot free (producer) 1 TMA issued | 2 tile landed (consumer) 9 operands in registers 7 MMAs retired 5 stage released
+    // 0 slot free (producer) 1 TMA issued | 2 tile landed (consumer) 9 operands in registers 5 stage released 7 MMAs committed
     long long* utr = nullptr;
     int utr_i = 0;
 #define UTR(k) do { if (utr && utr_i < 16) utr[utr_i * 16 + (k)] = clock64(); } while (0)
@@ -280,7 +308,7 @@ __global__ void __launch_bounds__(STC_THREADS, 1) sd_tc_kernel(const __grid_cons
         mbar_wait(smem_u32(&s_sfree[g.s]), g.sp ^ 1u);
         if (lane == 0) UTR(0);
         const uint32_t full = smem_u32(&s_full[g.s]);
-        mbar_expect_tx_elect(full, STC_A_BYTES);
+        mbar_expect_tx_elect(full, STC_STAGE_BYTES);
         tma_load_3d_elect(base_u32 + g.s * STC_STAGE_BYTES, map, full, c0, c1, c2);
         if (lane == 0) UTR(1);
     };
@@ -305,8 +333,9 @@ __global__ void __launch_bounds__(STC_THREADS, 1) sd_tc_kernel(const __grid_cons
                 ah[ks][r] = __float_as_uint(h); al[ks][r] = __float_as_uint(l);
             }
     };
-    // consumer: the three products of one unit against the B tile at b_hi (B_lo 2 KB behind it), then wait for them to retire
-    auto mma_unit = [&](float (&acc)[8], float (&acc2)[8], const uint32_t (&ah)[4][4], const uint32_t (&al)[4][4], uint32_t b_hi) {
+    // consumer: the three products of one unit against the B tile at b_hi (B_lo 2 KB behind it), committed as one group; the
+    // fragment registers stay read until the group retires
+    auto mma_issue = [&](float (&acc)[8], float (&acc2)[8], const uint32_t (&ah)[4][4], const uint32_t (&al)[4][4], uint32_t b_hi) {
         wgmma_fence();
 #pragma unroll
         for (int ks = 0; ks < 4; ++ks) {
@@ -316,12 +345,24 @@ __global__ void __launch_bounds__(STC_THREADS, 1) sd_tc_kernel(const __grid_cons
             wgmma_rs_n16(acc, ah[ks], dh);
         }
         wgmma_commit();
+    };
+    auto mma_drain = [&](float (&acc)[8], float (&acc2)[8]) {
         wgmma_wait<0>();
         wg_reg_fence(acc); wg_reg_fence(acc2);
     };
     auto release = [&](const Stage& g) {
         __syncwarp();
         if (lane == 0) mbar_arrive(smem_u32(&s_sfree[g.s]));
+    };
+    // consumer: wait for the unit in stage g, take its fragments into registers, free the stage, advance g
+    auto fetch = [&](Stage& g, bool transposed, uint32_t (&ah)[4][4], uint32_t (&al)[4][4]) {
+        mbar_wait(smem_u32(&s_full[g.s]), g.sp);
+        if (ct == 0) UTR(2);
+        load_frags(base + (size_t)g.s * STC_STAGE_BYTES, transposed, ah, al);
+        if (ct == 0) UTR(9);
+        release(g);
+        if (ct == 0) UTR(5);
+        stage_next(g);
     };
 
     // unit coordinates: adjoint sweep (chunk, sample, pixel block), apply sweep (sample, pixel tile, channel block)
@@ -374,15 +415,16 @@ __global__ void __launch_bounds__(STC_THREADS, 1) sd_tc_kernel(const __grid_cons
                 float acc[8], acc2[8];
 #pragma unroll
                 for (int i = 0; i < 8; ++i) { acc[i] = 0.f; acc2[i] = 0.f; }
-                for (int i = 0; i < nun; ++i) {
+                uint32_t ah0[4][4], al0[4][4], ah1[4][4], al1[4][4];
+                // unit i with its fragments in (ah, al): issue its MMAs, then load unit i+1 into (nh, nl) once unit i-1's MMAs
+                // (the last readers of (nh, nl)) have retired
+                auto step = [&](int i, const uint32_t (&ah)[4][4], const uint32_t (&al)[4][4], uint32_t (&nh)[4][4], uint32_t (&nl)[4][4]) {
                     const bool seg_first = (i == 0 || c.kb == 0), seg_last = (i == nun - 1 || c.kb == kba - 1);
                     if (seg_first) kb_first = c.kb;
-                    mbar_wait(smem_u32(&s_full[g.s]), g.sp);
-                    uint32_t ah[4][4], al[4][4];
-                    load_frags(base + (size_t)g.s * STC_STAGE_BYTES, true, ah, al);
-                    release(g);                                   // A is in registers, B (F^T) lives outside the stages
-                    mma_unit(acc, acc2, ah, al, ftb_m + (uint32_t)c.kb * 4096u);
+                    mma_issue(acc, acc2, ah, al, ftb_m + (uint32_t)c.kb * 4096u);
+                    if (i + 1 < nun) { wgmma_wait<1>(); fetch(g, true, nh, nl); }
                     if (seg_last) {
+                        mma_drain(acc, acc2);
                         // T[p][tap] of the finished segment: registers -> Tt[tap][p] -> shift-add over the taps -> qslots
 #pragma unroll
                         for (int j = 0; j < 2; ++j)
@@ -409,8 +451,14 @@ __global__ void __launch_bounds__(STC_THREADS, 1) sd_tc_kernel(const __grid_cons
                         }
                         asm volatile("bar.sync 1, %0;" ::"n"(STC_CT) : "memory");
                     }
-                    stage_next(g); app_next(c);
+                    app_next(c);
+                };
+                fetch(g, true, ah0, al0);
+                for (int i = 0; i < nun; i += 2) {
+                    step(i, ah0, al0, ah1, al1);
+                    if (i + 1 < nun) step(i + 1, ah1, al1, ah0, al0);
                 }
+                mma_drain(acc, acc2);                        // (already drained by the last unit; ptxas needs it to see that)
             }
         }
         ucount += (uint32_t)nun;
@@ -429,49 +477,22 @@ __global__ void __launch_bounds__(STC_THREADS, 1) sd_tc_kernel(const __grid_cons
                 produce_adj_run(ucount + (uint32_t)pf_adj, pf_adj, nun, true);
                 if (xpf) produce_apply_run(ucount + (uint32_t)nun, 0, min(NS, a_hi - a_lo));   // an apply sweep always follows an adjoint sweep
             } else {
-                const int tap = ct >> 4, kk0 = (ct & 15) * 2;             // this thread's two R^T elements: (tap, kk0 .. kk0 + 1)
-                const int dy = tap >> 2, dx = tap & 3;
-                const uint32_t boff = sw128(tap, kk0);
+                const uint32_t rt_m = smem_u32(ftb);
                 Stage g = stage_of(ucount);
-                AdjPos c = adj_pos(t_lo);
-                int j = 0, jsmp = -1;
+                int sl = 0;                                              // R^T pair slot of the unit (see build_rt)
                 int cl = 0, left = (chunk0 + 1) * per_chunk - t_lo;      // units left in the current chunk
                 float acc[8], acc2[8];
 #pragma unroll
                 for (int i = 0; i < 8; ++i) { acc[i] = 0.f; acc2[i] = 0.f; }
-                for (int i = 0; i < nun; ++i) {
-                    utr_i = i;
-                    // this thread's two elements of R^T for the unit (gathered from the mapped residual of the unit's sample)
-                    if (c.smp != jsmp) {                               // state slot of the sample
-                        j = 0;
-                        for (int jj = 1; jj < ns; ++jj) j = (s_state[jj] == c.smp) ? jj : j;
-                        jsmp = c.smp;
-                    }
-                    float rv[2];
-#pragma unroll
-                    for (int h = 0; h < 2; ++h) {
-                        const int px = c.kb * 32 + kk0 + h;
-                        const int iy = px / FS, ix = px - iy * FS;
-                        const int oy = iy - dy + 2, ox = ix - dx + 2;
-                        rv[h] = (px < NPX && oy >= 0 && oy < OS && ox >= 0 && ox < OS) ? sT[j * NPOS + oy * OS + ox] : 0.f;
-                    }
-                    mbar_wait(smem_u32(&s_full[g.s]), g.sp);
-                    if (ct == 0) UTR(2);
-                    uint8_t* sb = base + (size_t)g.s * STC_STAGE_BYTES;
-                    float2 bh, bl;
-                    split_tf32(rv[0], bh.x, bl.x); split_tf32(rv[1], bh.y, bl.y);
-                    *reinterpret_cast<float2*>(sb + STC_A_BYTES + boff) = bh;
-                    *reinterpret_cast<float2*>(sb + STC_A_BYTES + 2048 + boff) = bl;
-                    uint32_t ah[4][4], al[4][4];
-                    load_frags(sb, false, ah, al);
-                    if (ct == 0) UTR(9);
-                    asm volatile("fence.proxy.async.shared::cta;" ::: "memory");   // B tile (generic-proxy writes) -> visible to wgmma
-                    asm volatile("bar.sync 1, %0;" ::"n"(STC_CT) : "memory");
-                    mma_unit(acc, acc2, ah, al, smem_u32(sb + STC_A_BYTES));
+                uint32_t ah0[4][4], al0[4][4], ah1[4][4], al1[4][4];
+                // as in the apply sweep: issue unit i, then load unit i+1 into the other register set once unit i-1 has retired
+                auto step = [&](int i, const uint32_t (&ah)[4][4], const uint32_t (&al)[4][4], uint32_t (&nh)[4][4], uint32_t (&nl)[4][4]) {
+                    mma_issue(acc, acc2, ah, al, rt_m + (uint32_t)sl * 4096u);
                     if (ct == 0) UTR(7);
-                    release(g);
-                    if (ct == 0) UTR(5);
+                    if (++sl == per_chunk) sl = 0;
+                    if (i + 1 < nun) { wgmma_wait<1>(); utr_i = i + 1; fetch(g, false, nh, nl); }
                     if (--left == 0 || i == nun - 1) {
+                        mma_drain(acc, acc2);
                         // the chunk's partial gradient: rows = channels of the chunk, columns = taps
                         float* dst = Q.gpart + ((size_t)b * STC_MAXCH + cl) * 128 * 16;
 #pragma unroll
@@ -485,8 +506,14 @@ __global__ void __launch_bounds__(STC_THREADS, 1) sd_tc_kernel(const __grid_cons
                             }
                         ++cl; left = per_chunk;
                     }
-                    stage_next(g); adj_next(c);
+                };
+                utr_i = 0;
+                fetch(g, false, ah0, al0);
+                for (int i = 0; i < nun; i += 2) {
+                    step(i, ah0, al0, ah1, al1);
+                    if (i + 1 < nun) step(i + 1, ah1, al1, ah0, al0);
                 }
+                mma_drain(acc, acc2);                        // (already drained by the last unit; ptxas needs it to see that)
             }
         }
         ucount += (uint32_t)nun;
@@ -592,6 +619,7 @@ __global__ void __launch_bounds__(STC_THREADS, 1) sd_tc_kernel(const __grid_cons
         __syncthreads();
 
         SD_STAMP(tb + 1);
+        build_rt();
         utr = (P.trace && b == 0 && it == 0) ? reinterpret_cast<long long*>(P.trace) + 128 : nullptr;
         sweep_adjoint();
         utr = nullptr;
@@ -628,6 +656,7 @@ __global__ void __launch_bounds__(STC_THREADS, 1) sd_tc_kernel(const __grid_cons
         gl = block_sum(gl, s_red);
         if (tid == 0) Q.gnpart[b] = gl;
         grid_barrier(Q.barrier, epoch);
+        SD_STAMP(tb + 9);
         build_ft(Q.gfinal);
         SD_STAMP(tb + 4);
         sweep_apply(it + 1 < P.num_iter);
@@ -747,7 +776,10 @@ int launch_sd_tc(const SdParams& P0, cudaStream_t st, int* handled) {
     }
     if (smax > 16) return 0;
     const int slice_max = (C * 4 + G - 1) / G + 1;
-    const size_t fixed = 1024 + (size_t)kba * 4096 + 16 * STC_TT_PITCH * 4 + 2 * (size_t)slice_max * 16 +
+    // the B-tile region holds F^T (kba tiles) in the apply sweep and R^T of the adjoint range's (sample, pixel block) pairs in
+    // the adjoint sweep: min(longest range, n KBT) tiles
+    const int nbt = std::max(kba, (int)std::min((UT + G - 1) / G, (long long)n * KBT));
+    const size_t fixed = 1024 + (size_t)nbt * 4096 + 16 * STC_TT_PITCH * 4 + 2 * (size_t)slice_max * 16 +
                          (size_t)smax * 6 * NPOS * 4 + (size_t)smax * (STC_QL_MAX + 1) * 4 + 64;
     const size_t limit = 227 * 1024 - 3072;                     // static shared memory of the kernel: ~2.3 KB
     if (fixed + (size_t)STC_NS_MIN * STC_STAGE_BYTES > limit) return 0;
@@ -760,7 +792,7 @@ int launch_sd_tc(const SdParams& P0, cudaStream_t st, int* handled) {
     memset(&Q, 0, sizeof(Q));
     Q.p = P0;
     Q.p.trace = getenv("B200TRK_SD_TRACE") ? (unsigned long long*)workspace(4096, 3) : nullptr;
-    Q.smax = smax; Q.nchk = nchk; Q.kba = kba; Q.slice_max = slice_max; Q.ns = nstg;
+    Q.smax = smax; Q.nchk = nchk; Q.kba = kba; Q.slice_max = slice_max; Q.ns = nstg; Q.nbt = nbt;
 
     {
         // (the pixel dimension stays H*W whatever the pitch: reads past it are TMA zero fill, never the pitch padding)

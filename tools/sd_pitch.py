@@ -8,7 +8,7 @@ from pytracking_b200.frame_engine import DiMPFrameEngine
 
 def trace(tag):
     torch.cuda.synchronize()
-    buf = (C.c_uint64 * 64)()
+    buf = (C.c_uint64 * 128)()
     _lib.check(_lib.lib().b200trk_debug_sd_trace(buf))
     t = np.array(list(buf), dtype=np.float64)
     b = 8 + 10

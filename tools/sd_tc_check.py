@@ -57,7 +57,7 @@ w0 = torch.zeros(1, 512, 4, 4).cuda()
 for _ in range(4):
     ops.dimp_sd_gn(w0, feat, bb, sw, *luts, 4, 0.9, 0.01)
 torch.cuda.synchronize()
-buf = (C.c_uint64 * 64)()
+buf = (C.c_uint64 * 128)()
 _lib.check(_lib.lib().b200trk_debug_sd_trace(buf))
 t = np.array(list(buf), dtype=np.float64)
 print("prologue %.2f | s0 sweep %.2f | barrier %.2f | s-sum %.2f" % ((t[1]-t[0])/1e3, (t[2]-t[1])/1e3, (t[3]-t[2])/1e3, (t[4]-t[3])/1e3))
