@@ -278,6 +278,11 @@ double b200trk_net_flops(const b200trk_net_t* net);
  * and a device-to-device copy of a step's NHWC output activation [S,Hout,Wout,Cout] after a forward pass. */
 int b200trk_net_num_ops(const b200trk_net_t* net);
 int b200trk_net_op_info(const b200trk_net_t* net, int index, int info[8]);
+/* Operand wiring of a step: io = {step that produced its input, step that produced its residual or -1, relu, pad} (-1 also when the
+ * input is the caller's crop). And, for a convolution step (kind 3), a device-to-device copy of the weights it runs with: BN folded,
+ * repacked to [Cout][k][k][Cin], and of the bias [Cout]; b_dst is left untouched when the layer has no bias. Neither call changes the plan or drops a recorded CUDA graph. */
+int b200trk_net_op_io(const b200trk_net_t* net, int index, int io[4]);
+int b200trk_net_op_weights(const b200trk_net_t* net, int index, float* w_dst, float* b_dst, b200trk_stream_t stream);
 int b200trk_net_op_output(const b200trk_net_t* net, int index, int S, float* dst, b200trk_stream_t stream);
 /* Profiling aid for tensor-core steps: attach a DEVICE buffer of [ctas][8] uint64 per-CTA phase time stamps
  * (globaltimer ns: start, prologue done, previous grid complete, first operands landed, accumulator complete,

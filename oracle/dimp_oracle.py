@@ -112,18 +112,18 @@ def _padded_windows(feat, k):
 
 
 def apply_filter(feat, w):
-    """ltr/models/layers/filter.py:5-57 for one sequence: feat [n,C,H,W], w [1,C,k,k] -> [n,1,Ho,Wo],
+    """ltr/models/layers/filter.py:5-57 for one sequence: feat [n,C,H,W], w [1,C,k,k] -> [n,1,Ho,Wo] in feat's dtype,
     s[i,y,x] = sum_{c,u,v} xpad[i,c,y+u,x+v] * w[c,u,v], pad k//2 on all sides (19x19 for 18x18, k=4)."""
     k = w.shape[-1]
     win = _padded_windows(feat, k)
-    return torch.einsum("ncyxuv,cuv->nyx", win.double(), w[0].double()).float().unsqueeze(1)
+    return torch.einsum("ncyxuv,cuv->nyx", win.double(), w[0].double()).to(feat.dtype).unsqueeze(1)
 
 
 def apply_feat_transpose(feat, r, k):
     """ltr/models/layers/filter.py:91-107,129-182 (v2 and v3 are the same exact adjoint):
     g[c,u,v] = sum_{i,y,x} r[i,y,x] * xpad[i,c,y+u,x+v]. r is [n,1,Ho,Wo]; returns [1,C,k,k]."""
     win = _padded_windows(feat, k)
-    return torch.einsum("ncyxuv,nyx->cuv", win.double(), r[:, 0].double()).float().unsqueeze(0)
+    return torch.einsum("ncyxuv,nyx->cuv", win.double(), r[:, 0].double()).to(feat.dtype).unsqueeze(0)
 
 
 def max2d(a):
@@ -152,8 +152,8 @@ def dimp_label_maps(bb, params, out_sz, filter_size=4, feat_stride=16, bin_displ
     """optimizer.py:111-119: label y, target mask m = sigmoid(.), spatial weight v per sample; [n,Ho,Wo] each."""
     off = (filter_size % 2) / 2.0
     center = ((bb[:, :2] + bb[:, 2:] / 2) / feat_stride).flip((1,)) - off   # (row, col)
-    k0 = torch.arange(out_sz[0], dtype=torch.float32).view(1, -1, 1)
-    k1 = torch.arange(out_sz[1], dtype=torch.float32).view(1, 1, -1)
+    k0 = torch.arange(out_sz[0], dtype=bb.dtype).view(1, -1, 1)
+    k1 = torch.arange(out_sz[1], dtype=bb.dtype).view(1, 1, -1)
     d0 = k0 - center[:, 0].view(-1, 1, 1)
     d1 = k1 - center[:, 1].view(-1, 1, 1)
     rho = torch.sqrt(d0 * d0 + d1 * d1) / bin_displacement

@@ -121,6 +121,8 @@ SIGNATURES = {
     "b200trk_net_flops": (C.c_double, [_VP]),
     "b200trk_net_num_ops": (_I, [_VP]),
     "b200trk_net_op_info": (_I, [_VP, _I, C.POINTER(C.c_int * 8)]),
+    "b200trk_net_op_io": (_I, [_VP, _I, C.POINTER(C.c_int * 4)]),
+    "b200trk_net_op_weights": (_I, [_VP, _I, _VP, _VP, _VP]),
     "b200trk_net_op_output": (_I, [_VP, _I, _I, _VP, _VP]),
     "b200trk_net_op_set_timing_buffer": (_I, [_VP, _I, _VP]),
     "b200trk_net_op_grid": (_I, [_VP, _I, C.POINTER(C.c_int * 4)]),

@@ -274,6 +274,31 @@ extern "C" int b200trk_net_op_info(const b200trk_net_t* net, int index, int info
     return 0;
 }
 
+// plan step whose output lives in activation buffer `buf` (each step writes a buffer of its own), -1 when none does
+static int producer_of(const b200trk_net_t* net, int buf) {
+    if (buf < 0) return -1;
+    for (int i = 0; i < (int)net->ops.size(); ++i)
+        if (net->ops[i].out == buf) return i;
+    return -1;
+}
+
+extern "C" int b200trk_net_op_io(const b200trk_net_t* net, int index, int io[4]) {
+    B200_REQUIRE(net && io && index >= 0 && index < (int)net->ops.size(), "net_op_io: bad argument");
+    const Op& op = net->ops[index];
+    io[0] = producer_of(net, op.in); io[1] = producer_of(net, op.res); io[2] = op.relu; io[3] = op.pad;
+    return 0;
+}
+
+extern "C" int b200trk_net_op_weights(const b200trk_net_t* net, int index, float* w_dst, float* b_dst, b200trk_stream_t stream) {
+    B200_REQUIRE(net && w_dst && index >= 0 && index < (int)net->ops.size() && net->ops[index].kind == OP_CONV,
+                 "net_op_weights: bad argument");
+    const Op& op = net->ops[index];
+    cudaStream_t st = (cudaStream_t)stream;
+    B200_CHECK_CUDA(cudaMemcpyAsync(w_dst, op.w, (size_t)op.Cout * op.k * op.k * op.Cin * sizeof(float), cudaMemcpyDeviceToDevice, st));
+    if (op.bias && b_dst) B200_CHECK_CUDA(cudaMemcpyAsync(b_dst, op.bias, (size_t)op.Cout * sizeof(float), cudaMemcpyDeviceToDevice, st));
+    return 0;
+}
+
 extern "C" int b200trk_net_op_output(const b200trk_net_t* net, int index, int S, float* dst, b200trk_stream_t stream) {
     B200_REQUIRE(net && dst && index >= 0 && index < (int)net->ops.size(), "net_op_output: bad argument");
     const Op& op = net->ops[index];
