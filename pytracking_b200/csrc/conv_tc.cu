@@ -19,8 +19,8 @@
 // Epilogue: registers -> shared-memory staging tile -> bias/residual/ReLU -> coalesced global stores. Small layers use split-K over
 // gridDim.z: the <= 8 split CTAs of a tile form a thread-block cluster, stage their partial tiles in their own shared memory and each
 // reduces its share of the tile through distributed shared memory in split order (fixed order => bitwise deterministic); with more
-// than 8 splits (or B200TRK_TC_CLUSTER=0) the partial tiles go to an L2-resident workspace and a per-tile arrival counter releases
-// the split CTAs.
+// than 8 splits, when the device cannot hold all of the grid's clusters at once, or with B200TRK_TC_CLUSTER=0, the partial tiles go
+// to an L2-resident workspace and a per-tile arrival counter releases the split CTAs.
 #include "net.cuh"
 #include "tc_ptx.cuh"
 #include <cuda.h>
@@ -451,6 +451,39 @@ int tc_conv_prepare(b200trk_net* net, Op& op, const std::vector<float>& w_khwc) 
     return 0;
 }
 
+static int tc_set_kernel_attrs() {
+    static bool attr = false;
+    if (!attr) {
+        B200_CHECK_CUDA(cudaFuncSetAttribute(conv_tc_kernel<64>, cudaFuncAttributeMaxDynamicSharedMemorySize, TC_SMEM_MAX));
+        B200_CHECK_CUDA(cudaFuncSetAttribute(conv_tc_kernel<128>, cudaFuncAttributeMaxDynamicSharedMemorySize, TC_SMEM_MAX));
+        attr = true;
+    }
+    return 0;
+}
+
+static size_t tc_smem_bytes(const TcParams& P) {
+    size_t smem = (size_t)P.stages * P.stage_bytes + 1024;
+    const size_t staging = (size_t)TC_BM * (P.BN + 4) * sizeof(float) + 1024;    // the epilogue's accumulator tile
+    return smem < staging ? staging : smem;
+}
+
+// How many (1, 1, splits) clusters of this configuration the device can hold at once. A cluster's CTAs must share a GPC, so
+// sizes that do not divide a GPC's SM count leave SMs idle: on a 132-SM H100, 44 clusters of 3 or 24 of 5 do not all fit, and
+// the last clusters run as a second wave that costs a whole CTA lifetime.
+static int tc_max_active_clusters(const TcParams& P, int ctas, int* n) {
+    if (int e = tc_set_kernel_attrs()) return e;
+    cudaLaunchConfig_t cfg;
+    memset(&cfg, 0, sizeof(cfg));
+    cfg.gridDim = dim3(ctas, 1, P.splits); cfg.blockDim = dim3(TC_THREADS); cfg.dynamicSmemBytes = tc_smem_bytes(P);
+    cudaLaunchAttribute at;
+    at.id = cudaLaunchAttributeClusterDimension;
+    at.val.clusterDim.x = 1; at.val.clusterDim.y = 1; at.val.clusterDim.z = (unsigned)P.splits;
+    cfg.attrs = &at; cfg.numAttrs = 1;
+    if (P.BN == 64) B200_CHECK_CUDA(cudaOccupancyMaxActiveClusters(n, conv_tc_kernel<64>, &cfg));
+    else B200_CHECK_CUDA(cudaOccupancyMaxActiveClusters(n, conv_tc_kernel<128>, &cfg));
+    return 0;
+}
+
 // per-batch-size launch geometry (BN, split-K); the weight tensor maps depend on BN
 static int tc_configure(b200trk_net* net, const Op& op, TcConv* tc, int S) {
     TcParams& P = tc->P;
@@ -498,6 +531,14 @@ static int tc_configure(b200trk_net* net, const Op& op, TcConv* tc, int S) {
     B200_REQUIRE(ctas <= 512 || P.splits == 1, "tc_conv: counter array too small for %d tiles", ctas);
     P.ws = op.side ? net->splitk_ws2 : net->splitk_ws;
     P.cluster_red = (env_int("B200TRK_TC_CLUSTER", 1) && P.splits > 1 && P.splits <= 8) ? 1 : 0;
+    if (P.cluster_red) {
+        // Clusters that cannot all be resident at once reduce through the L2 workspace instead, as one wave of plain CTAs. Both
+        // reductions add the same staged partial tiles in split order from 0.f, padded with zeros to 8 terms, so the output is
+        // bitwise the same.
+        int fit = 0;
+        if (int e = tc_max_active_clusters(P, ctas, &fit)) return e;
+        if (fit < ctas) P.cluster_red = 0;
+    }
     P.prefetch_b = env_int("B200TRK_TC_PREFETCH_B", 1);
     const size_t Kt = (size_t)op.k * op.k * op.Cin;
     if (int e = make_map_2d(&P.b_map, op.w, Kt, op.Cout, BN)) return e;
@@ -510,15 +551,8 @@ int tc_conv_launch(b200trk_net* net, const Op& op, int S, cudaStream_t st) {
     if (tc->S_built != S)
         if (int e = tc_configure(net, op, tc, S)) return e;
     const TcParams& P = tc->P;
-    size_t smem = (size_t)P.stages * P.stage_bytes + 1024;
-    const size_t staging = (size_t)TC_BM * (P.BN + 4) * sizeof(float) + 1024;    // the epilogue's accumulator tile
-    if (smem < staging) smem = staging;
-    static bool attr = false;
-    if (!attr) {
-        B200_CHECK_CUDA(cudaFuncSetAttribute(conv_tc_kernel<64>, cudaFuncAttributeMaxDynamicSharedMemorySize, TC_SMEM_MAX));
-        B200_CHECK_CUDA(cudaFuncSetAttribute(conv_tc_kernel<128>, cudaFuncAttributeMaxDynamicSharedMemorySize, TC_SMEM_MAX));
-        attr = true;
-    }
+    const size_t smem = tc_smem_bytes(P);
+    if (int e = tc_set_kernel_attrs()) return e;
     dim3 grid(P.tiles_w * P.tiles_h * S, op.Cout / P.BN, P.splits);
     cudaLaunchConfig_t cfg;
     memset(&cfg, 0, sizeof(cfg));
