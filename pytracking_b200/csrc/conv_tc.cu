@@ -3,19 +3,25 @@
 //
 //   D[m][n] = sum_k A[m][k] * W[n][k]     m = output pixel, n = output channel, k = (kh, kw, cin)
 //
-// fp32 fidelity on a TF32 datapath: every operand tile is split into a (hi, lo) pair of TF32-representable fp32 numbers,
+// fp32 fidelity on a TF32 datapath: every operand is split into a (hi, lo) pair of TF32-representable fp32 numbers,
 // x = hi + lo (+ <= 2^-22 |x|), and each K step issues three MMAs: A_lo*B_hi + A_hi*B_lo into one fp32 accumulator and A_hi*B_hi
-// into another (summed in the epilogue) ("3xTF32"); the dropped A_lo*B_lo term is O(2^-22) relative. HBM/L2 only ever hold (and
-// move) plain fp32 activations and weights.
+// into another (summed in the epilogue) ("3xTF32"); the dropped A_lo*B_lo term is O(2^-22) relative. The weights are split once
+// when the plan is built (tc_conv_prepare: a [2][Cout][K] hi | lo copy next to the raw op.w); the activations stay plain fp32 in
+// HBM / L2 and are split after they land in shared memory.
 //
 // Tiling: CTA = 128 output pixels (a BW x BH rectangle of one sample, rows ordered (y, x)) x BN output channels (64 or 128).
 // K is walked in 128-byte blocks (32 input channels of one filter tap): one 4-D TMA box {32 ch, BW*stride, BH*stride, 1}
-// (element strides {1, stride, stride, 1}; halo / padding = TMA out-of-bounds zero fill) lands the A tile in the K-major
-// SWIZZLE_128B layout; a 2-D box {32, BN} does the same for the weights. Warp roles: warps 0-7 = two consumer warpgroups (rows
-// 0-63 and 64-127 of the tile), warp 8 = TMA producer. A consumer k-block: wait for the stage, split the raw tiles in place
-// (hi over the raw value, lo into the neighbouring slot; element-wise, so the swizzle is irrelevant), make the writes visible to
-// the async proxy, meet the other warpgroup, issue 12 wgmmas (4 K steps x 3 products) and release the PREVIOUS stage once its
-// wgmma group has retired, so that the split of one k-block overlaps the MMAs of the one before.
+// (element strides {1, stride, stride, 1}; halo / padding = TMA out-of-bounds zero fill) lands the raw A tile in the K-major
+// SWIZZLE_128B layout; a 3-D box {32, BN, 2} lands B_hi and, BN * 128 bytes behind it, B_lo in the same layout. Warp roles: warps
+// 0-7 = two consumer warpgroups (rows 0-63 and 64-127 of the tile), warp 8 = TMA producer. A consumer k-block issues 12 wgmmas
+// (4 K steps x 3 products), waits until only that group is in flight and releases the stage of the retired group; the two
+// warpgroups never meet inside the K loop.
+//   BN = 64: A from registers. After the release the consumer waits for the next stage and loads + splits its own rows' A fragments
+//            into the other of two register sets, so the fragment load of one k-block overlaps the MMAs of the one before; no
+//            thread writes the stages.
+//   BN = 128: A from shared memory. Each warpgroup splits its own 64 rows of the raw tile in place (hi over the raw value, lo into
+//            an A_lo slot), fences them for the async proxy and meets its own 4 warps before its MMAs. The 128 accumulators leave
+//            no room for two fragment sets: 9 warps put 3 on one SM sub-partition, whose 16384 registers cap a thread at 168.
 // Epilogue: registers -> shared-memory staging tile -> bias/residual/ReLU -> coalesced global stores. Small layers use split-K over
 // gridDim.z: the <= 8 split CTAs of a tile form a thread-block cluster, stage their partial tiles in their own shared memory and each
 // reduces its share of the tile through distributed shared memory in split order (fixed order => bitwise deterministic); with more
@@ -37,7 +43,7 @@ constexpr int TC_MAX_STAGES = 6;
 constexpr int TC_SMEM_MAX = 220 * 1024;
 
 struct TcParams {
-    CUtensorMap a_map, b_map;       // raw fp32 activations (4-D) and weights (2-D)
+    CUtensorMap a_map, b_map;       // raw fp32 activations (4-D) and TF32-split weights (3-D: K, Cout, hi | lo)
     float* out_raw;
     const float* bias; const float* residual;
     float* ws; unsigned* counters;
@@ -52,11 +58,12 @@ struct TcParams {
                      //    distributed shared memory instead of an L2 workspace + arrival counter
     int prefetch_b;  // 1: the weight tiles of the first pipeline stages are requested before griddepcontrol.wait (they do not depend on the previous layer)
     uint32_t stage_bytes;
-    uint32_t a_bytes, b_bytes;
+    uint32_t a_bytes, b_bytes;      // bytes one k-block's TMA lands: the A box | the B_hi and B_lo tiles
 };
 
 struct TcConv {
     TcParams P;
+    float* w_split = nullptr;       // [2][Cout][K]: TF32 hi | lo of the weights, the B operand (owned by the plan)
     int S_built = 0;
 };
 
@@ -88,10 +95,14 @@ __device__ __forceinline__ float4 ld_dsmem_f4(uint32_t local_addr, uint32_t rank
     return v;
 }
 
-template <int BN>
-__device__ __forceinline__ void tc_mma(float (&d)[BN / 2], uint64_t a, uint64_t b) {
-    if constexpr (BN == 64) wgmma_ss_n64(d, a, b);
-    else wgmma_ss_n128(d, a, b);
+// TF32 split of the weights, once per plan: hl[0][i] = hi, hl[1][i] = lo of w[i] (the same split_tf32 the activations get)
+__global__ void tc_split_weights_kernel(const float* __restrict__ w, float* __restrict__ hl, size_t n) {
+    for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x) {
+        float h, l;
+        split_tf32(w[i], h, l);
+        hl[i] = h;
+        hl[n + i] = l;
+    }
 }
 
 template <int BN>
@@ -99,7 +110,10 @@ __global__ void __launch_bounds__(TC_THREADS, 1) conv_tc_kernel(const __grid_con
     constexpr int NACC = BN / 2;                 // accumulator registers per thread and product group
     constexpr uint32_t a_tile = (uint32_t)TC_BM * 128u;   // 16 KB slot regardless of the box size
     constexpr uint32_t b_tile = (uint32_t)BN * 128u;
-    constexpr uint32_t b_off = 2u * a_tile;     // stage = A_hi | A_lo | B_hi | B_lo
+    // BN = 64: A from registers, stage = A (raw) | B_hi | B_lo. BN = 128: A from shared memory, split in place by the warpgroup that
+    // reads it, stage = A_hi | A_lo | B_hi | B_lo (see the header)
+    constexpr bool a_smem = BN == 128;
+    constexpr uint32_t b_off = (a_smem ? 2u : 1u) * a_tile;
     constexpr int RP = BN + 4;                   // floats per staged accumulator row (conflict-free 128-bit accesses)
     extern __shared__ uint8_t tc_smem_raw[];
     __shared__ __align__(8) uint64_t s_full[TC_MAX_STAGES];
@@ -146,7 +160,7 @@ __global__ void __launch_bounds__(TC_THREADS, 1) conv_tc_kernel(const __grid_con
         for (int it = 0; it < npre; ++it) {
             const uint32_t full = smem_u32(&s_full[it]);
             mbar_expect_tx_elect(full, P.a_bytes + P.b_bytes);
-            tma_load_2d_elect(smem_base + (uint32_t)it * stage_bytes + b_off, &P.b_map, full, tap * P.Cin + cb * TC_KB, n0);
+            tma_load_3d_elect(smem_base + (uint32_t)it * stage_bytes + b_off, &P.b_map, full, tap * P.Cin + cb * TC_KB, n0, 0);
             if (++cb == P.cblks) { cb = 0; ++tap; }
         }
     }
@@ -167,61 +181,97 @@ __global__ void __launch_bounds__(TC_THREADS, 1) conv_tc_kernel(const __grid_con
                 mbar_expect_tx_elect(full, P.a_bytes + P.b_bytes);
             }
             const uint32_t sa = smem_base + (uint32_t)st * stage_bytes;
-            tma_load_4d_elect(sa, &P.a_map, full, cb * TC_KB, x0 + kw, y0 + kh, s);                    // raw -> A_hi slot
-            if (it >= npre) tma_load_2d_elect(sa + b_off, &P.b_map, full, tap * P.Cin + cb * TC_KB, n0);  // raw -> B_hi slot
+            tma_load_4d_elect(sa, &P.a_map, full, cb * TC_KB, x0 + kw, y0 + kh, s);                          // raw A
+            if (it >= npre) tma_load_3d_elect(sa + b_off, &P.b_map, full, tap * P.Cin + cb * TC_KB, n0, 0);  // B_hi | B_lo
             if (++cb == P.cblks) { cb = 0; ++tap; if (++kw == P.ksz) { kw = 0; ++kh; } }
             if (++st == P.stages) { st = 0; ph ^= 1u; }
         }
     } else {
-        // ===================== consumer warpgroups: operand split + wgmma, then the accumulator staging =====================
+        // ===================== consumer warpgroups: A fragments + wgmma, then the accumulator staging =====================
         const int ct = threadIdx.x, wg = ct >> 7;
+        const int r0 = wg * 64 + (warp & 3) * 16 + (lane >> 2), kq = lane & 3;     // this thread's fragment rows / K column
         float acc[NACC], acc2[NACC];                  // A_hi*B_hi | A_lo*B_hi + A_hi*B_lo
 #pragma unroll
         for (int i = 0; i < NACC; ++i) { acc[i] = 0.f; acc2[i] = 0.f; }
-        constexpr int NA = (int)(a_tile / 16) / TC_CT, NB = (int)(b_tile / 16) / TC_CT;     // float4 per thread: 4 | 2 or 4
-        int st = 0, prev = 0;
-        uint32_t ph = 0;
-        for (int it = 0; it < nkb; ++it) {
-            mbar_wait(smem_u32(&s_full[st]), ph);
-            if (dbg && it == 0 && ct == 0) dbg[3] = gtimer();             // first operands landed
-            float4* a_hi = reinterpret_cast<float4*>(sbase + (size_t)st * stage_bytes);
-            float4* a_lo = a_hi + a_tile / 16;
-            float4* b_hi = reinterpret_cast<float4*>(sbase + (size_t)st * stage_bytes + b_off);
-            float4* b_lo = b_hi + b_tile / 16;
-            // all loads of the stage are issued before the first store (the compiler must not serialise them behind the stores)
-            float4 xa[NA], xb[NB];
+        if constexpr (!a_smem) {
+            uint32_t ah0[4][4], al0[4][4], ah1[4][4], al1[4][4];    // two sets of A fragments (4 K steps), alternating by k-block
+            int st = 0, prev = 0;
+            uint32_t ph = 0;
+            // k-block `it`, its fragments in (ah, al) and its weight tiles in stage st: issue its 12 MMAs as one group. Once the
+            // previous k-block's group has retired, its stage goes back to the producer and k-block it + 1's fragments are loaded
+            // into (nh, nl), the registers that group read, while k-block it's group is in flight.
+            auto step = [&](int it, const uint32_t (&ah)[4][4], const uint32_t (&al)[4][4], uint32_t (&nh)[4][4], uint32_t (&nl)[4][4]) {
+                const uint32_t sb = smem_base + (uint32_t)st * stage_bytes + b_off;
+                wgmma_fence();
 #pragma unroll
-            for (int j = 0; j < NA; ++j) xa[j] = a_hi[ct + TC_CT * j];
-#pragma unroll
-            for (int j = 0; j < NB; ++j) xb[j] = b_hi[ct + TC_CT * j];
-#pragma unroll
-            for (int j = 0; j < NA; ++j) { float4 h, l; split_tf32_4(xa[j], h, l); a_hi[ct + TC_CT * j] = h; a_lo[ct + TC_CT * j] = l; }
-#pragma unroll
-            for (int j = 0; j < NB; ++j) { float4 h, l; split_tf32_4(xb[j], h, l); b_hi[ct + TC_CT * j] = h; b_lo[ct + TC_CT * j] = l; }
-            asm volatile("fence.proxy.async.shared::cta;" ::: "memory");     // generic-proxy writes -> visible to wgmma
-            asm volatile("bar.sync 1, %0;" ::"n"(TC_CT) : "memory");          // both warpgroups read all of B
-            const uint32_t sa = smem_base + (uint32_t)st * stage_bytes + (uint32_t)wg * 64u * 128u;   // this warpgroup's 64 rows
-            const uint32_t sb = smem_base + (uint32_t)st * stage_bytes + b_off;
-            wgmma_fence();
-#pragma unroll
-            for (int k = 0; k < TC_KB / 8; ++k) {
-                const uint32_t adv = (uint32_t)k * 32u;                       // 8 tf32 = 32 bytes per K step
-                tc_mma<BN>(acc2, wg_desc(sa + a_tile + adv), wg_desc(sb + adv));
-                tc_mma<BN>(acc2, wg_desc(sa + adv), wg_desc(sb + b_tile + adv));
-                tc_mma<BN>(acc, wg_desc(sa + adv), wg_desc(sb + adv));
+                for (int k = 0; k < TC_KB / 8; ++k) {
+                    const uint32_t adv = (uint32_t)k * 32u;                       // 8 tf32 = 32 bytes per K step
+                    const uint64_t dh = wg_desc(sb + adv), dl = wg_desc(sb + b_tile + adv);
+                    wgmma_rs_n64(acc2, al[k], dh);
+                    wgmma_rs_n64(acc2, ah[k], dl);
+                    wgmma_rs_n64(acc, ah[k], dh);
+                }
+                wgmma_commit();
+                wgmma_wait<1>();
+                if (it > 0 && lane == 0) mbar_arrive(smem_u32(&s_empty[prev]));
+                prev = st;
+                if (++st == P.stages) { st = 0; ph ^= 1u; }
+                if (it + 1 < nkb) {
+                    mbar_wait(smem_u32(&s_full[st]), ph);
+                    load_frags_split(sbase + (size_t)st * stage_bytes, r0, kq, 0, false, nh, nl);
+                }
+            };
+            mbar_wait(smem_u32(&s_full[0]), 0);
+            if (dbg && ct == 0) dbg[3] = gtimer();                            // first operands landed
+            load_frags_split(sbase, r0, kq, 0, false, ah0, al0);
+            for (int it = 0; it < nkb; it += 2) {
+                step(it, ah0, al0, ah1, al1);
+                if (it + 1 < nkb) step(it + 1, ah1, al1, ah0, al0);
             }
-            wgmma_commit();
-            wgmma_wait<1>();                       // the previous k-block's group has retired: its stage may be refilled
-            if (it > 0 && lane == 0) mbar_arrive(smem_u32(&s_empty[prev]));
-            prev = st;
-            if (++st == P.stages) { st = 0; ph ^= 1u; }
+        } else {
+            // each warpgroup splits its own 64 rows of A in place (hi over the raw value, lo into the A_lo slot; element-wise, so
+            // the swizzle is irrelevant) and meets only its own warps before its MMAs read them
+            const int wt = ct & 127;
+            int st = 0, prev = 0;
+            uint32_t ph = 0;
+            for (int it = 0; it < nkb; ++it) {
+                mbar_wait(smem_u32(&s_full[st]), ph);
+                if (dbg && it == 0 && ct == 0) dbg[3] = gtimer();         // first operands landed
+                float4* a_hi = reinterpret_cast<float4*>(sbase + (size_t)st * stage_bytes + (size_t)wg * 64 * 128);
+                float4* a_lo = a_hi + a_tile / 16;
+                float4 xa[4];
+#pragma unroll
+                for (int q = 0; q < 4; ++q) xa[q] = a_hi[wt + 128 * q];
+#pragma unroll
+                for (int q = 0; q < 4; ++q) { float4 h, l; split_tf32_4(xa[q], h, l); a_hi[wt + 128 * q] = h; a_lo[wt + 128 * q] = l; }
+                asm volatile("fence.proxy.async.shared::cta;" ::: "memory");  // generic-proxy writes -> visible to wgmma
+                if (wg == 0) asm volatile("bar.sync 2, 128;" ::: "memory");
+                else asm volatile("bar.sync 3, 128;" ::: "memory");
+                const uint32_t sa = smem_base + (uint32_t)st * stage_bytes + (uint32_t)wg * 64u * 128u;
+                const uint32_t sb = smem_base + (uint32_t)st * stage_bytes + b_off;
+                wgmma_fence();
+#pragma unroll
+                for (int k = 0; k < TC_KB / 8; ++k) {
+                    const uint32_t adv = (uint32_t)k * 32u;
+                    const uint64_t ah = wg_desc(sa + adv), al = wg_desc(sa + a_tile + adv);
+                    const uint64_t dh = wg_desc(sb + adv), dl = wg_desc(sb + b_tile + adv);
+                    wgmma_ss_n128(acc2, al, dh);
+                    wgmma_ss_n128(acc2, ah, dl);
+                    wgmma_ss_n128(acc, ah, dh);
+                }
+                wgmma_commit();
+                wgmma_wait<1>();                   // the previous k-block's group has retired: its stage may be refilled
+                if (it > 0 && lane == 0) mbar_arrive(smem_u32(&s_empty[prev]));
+                prev = st;
+                if (++st == P.stages) { st = 0; ph ^= 1u; }
+            }
         }
         wgmma_wait<0>();
         wg_reg_fence(acc); wg_reg_fence(acc2);
         if (dbg && ct == 0) dbg[4] = gtimer();                            // accumulator complete
         asm volatile("bar.sync 1, %0;" ::"n"(TC_CT) : "memory");              // every wgmma of both warpgroups has read its operands
         {
-            const int r0 = wg * 64 + ((ct & 127) >> 5) * 16 + (lane >> 2), c0 = 2 * (lane & 3);
+            const int c0 = 2 * (lane & 3);             // accumulator rows r0, r0 + 8: the fragment rows
 #pragma unroll
             for (int j = 0; j < BN / 8; ++j)
 #pragma unroll
@@ -381,19 +431,6 @@ int tc_make_map(CUtensorMap* m, float* base, int rank, const uint64_t* dims, con
     return 0;
 }
 
-static int make_map_2d(CUtensorMap* m, float* base, uint64_t K, uint64_t N, uint32_t boxN) {
-    EncodeTiledFn enc = get_encode_fn();
-    B200_REQUIRE(enc, "tc_conv: cuTensorMapEncodeTiled not available from the driver");
-    cuuint64_t dims[2] = {K, N};
-    cuuint64_t strides[1] = {K * sizeof(float)};
-    cuuint32_t box[2] = {TC_KB, boxN};
-    cuuint32_t es[2] = {1, 1};
-    CUresult r = enc(m, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 2, base, dims, strides, box, es, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                     CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-    B200_REQUIRE(r == CUDA_SUCCESS, "tc_conv: cuTensorMapEncodeTiled(weights K=%llu N=%llu) failed: %d", (unsigned long long)K, (unsigned long long)N, (int)r);
-    return 0;
-}
-
 static int make_map_4d(CUtensorMap* m, float* base, int C, int W, int H, int S, int boxW, int boxH, int stride) {
     EncodeTiledFn enc = get_encode_fn();
     B200_REQUIRE(enc, "tc_conv: cuTensorMapEncodeTiled not available from the driver");
@@ -424,7 +461,7 @@ static void pick_tile(int Wout, int Hout, int stride, int* BW, int* BH) {
 }
 
 int tc_conv_prepare(b200trk_net* net, Op& op, const std::vector<float>& w_khwc) {
-    (void)w_khwc;                    // the raw repacked weights (op.w) are the B operand; the TF32 split happens in the kernel
+    (void)w_khwc;                    // the repacked weights are read from op.w on the device
     TcConv* tc = new TcConv();
     op.tc = tc;
     TcParams& P = tc->P;
@@ -447,6 +484,17 @@ int tc_conv_prepare(b200trk_net* net, Op& op, const std::vector<float>& w_khwc) 
     B200_CHECK_CUDA(cudaMemset(cnt, 0, 1024 * sizeof(unsigned)));
     net->owned.push_back(cnt);
     P.counters = (unsigned*)cnt;
+    // The B operand: the weights split into TF32 hi | lo once, here, instead of in every CTA that loads them. op.w stays the raw
+    // fp32 weights (the plan's weight read-back and the exact-fp32 path use them).
+    const size_t nw = (size_t)op.Cout * op.k * op.k * op.Cin;
+    void* hl = nullptr;
+    B200_CHECK_CUDA(cudaMalloc(&hl, 2 * nw * sizeof(float)));
+    net->owned.push_back(hl);
+    tc->w_split = (float*)hl;
+    const size_t blocks = (nw + 255) / 256;
+    tc_split_weights_kernel<<<(unsigned)(blocks < 4096 ? blocks : 4096), 256>>>(op.w, tc->w_split, nw);
+    B200_CHECK_CUDA(cudaGetLastError());
+    B200_CHECK_CUDA(cudaStreamSynchronize(0));
     tc->S_built = -1;
     return 0;
 }
@@ -505,8 +553,9 @@ static int tc_configure(b200trk_net* net, const Op& op, TcConv* tc, int S) {
     }
     if (op.Cout % BN != 0 || (BN != 64 && BN != 128)) BN = 64;
     P.BN = BN;
-    P.b_bytes = (uint32_t)BN * 128u;
-    const uint32_t stage_bytes = 2u * TC_BM * 128u + 2u * P.b_bytes;     // A_hi | A_lo | B_hi | B_lo
+    P.b_bytes = 2u * (uint32_t)BN * 128u;                           // B_hi | B_lo
+    // BN 64: A | B_hi | B_lo, 32 KB (6 stages); BN 128: A_hi | A_lo | B_hi | B_lo, 64 KB (3 stages)
+    const uint32_t stage_bytes = (BN == 128 ? 2u : 1u) * TC_BM * 128u + P.b_bytes;
     P.stage_bytes = stage_bytes;
     int stages = (int)((TC_SMEM_MAX - 1024u) / stage_bytes);
     if (stages > TC_MAX_STAGES) stages = TC_MAX_STAGES;
@@ -540,8 +589,12 @@ static int tc_configure(b200trk_net* net, const Op& op, TcConv* tc, int S) {
         if (fit < ctas) P.cluster_red = 0;
     }
     P.prefetch_b = env_int("B200TRK_TC_PREFETCH_B", 1);
-    const size_t Kt = (size_t)op.k * op.k * op.Cin;
-    if (int e = make_map_2d(&P.b_map, op.w, Kt, op.Cout, BN)) return e;
+    // {K, Cout, hi | lo}: one box {32, BN, 2} lands B_hi and, BN * 128 bytes behind it, B_lo
+    const uint64_t Kt = (uint64_t)op.k * op.k * op.Cin;
+    const uint64_t bdims[3] = {Kt, (uint64_t)op.Cout, 2};
+    const uint64_t bstrides[2] = {Kt * sizeof(float), Kt * op.Cout * sizeof(float)};
+    const uint32_t bbox[3] = {TC_KB, (uint32_t)BN, 2};
+    if (int e = tc_make_map(&P.b_map, tc->w_split, 3, bdims, bstrides, bbox, 1)) return e;
     tc->S_built = S;
     return 0;
 }

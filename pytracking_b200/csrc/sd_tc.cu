@@ -65,10 +65,6 @@ __device__ __forceinline__ int part_lo(long long U, int G, int b) { return (int)
 __device__ __forceinline__ int part_owner(long long U, int G, int u) { return (int)((((long long)u + 1) * G - 1) / U); }
 
 __device__ __forceinline__ float tf32_lo(float x) { return tf32_rna(x - tf32_rna(x)); }
-// byte offset of element (row, k) inside a K-major SWIZZLE_128B tile of 128-byte rows (tile base 1024-byte aligned)
-__device__ __forceinline__ uint32_t sw128(int row, int k) {
-    return (uint32_t)(row * 128 + ((((k >> 2) ^ (row & 7)) << 4) | ((k & 3) << 2)));
-}
 __device__ __forceinline__ float warp_sum_xor(float v) {
 #pragma unroll
     for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
@@ -312,27 +308,6 @@ __global__ void __launch_bounds__(STC_THREADS, 1) sd_tc_kernel(const __grid_cons
         tma_load_3d_elect(base_u32 + g.s * STC_STAGE_BYTES, map, full, c0, c1, c2);
         if (lane == 0) UTR(1);
     };
-    // consumer: this thread's A fragments of the unit (4 K steps x 4 registers), split into hi / lo
-    auto load_frags = [&](const uint8_t* sb, bool transposed, uint32_t (&ah)[4][4], uint32_t (&al)[4][4]) {
-        float x[4][4];
-#pragma unroll
-        for (int ks = 0; ks < 4; ++ks) {
-#pragma unroll
-            for (int r = 0; r < 4; ++r) {
-                const int row = r0 + 8 * (r & 1), k = 8 * ks + kq + 4 * (r >> 1);
-                // adjoint: [128 rows][32 k] with the 128-byte swizzle; apply: [32 k][128 rows] linear (512-byte lines)
-                x[ks][r] = transposed ? reinterpret_cast<const float*>(sb)[k * 128 + row] : *reinterpret_cast<const float*>(sb + sw128(row, k));
-            }
-        }
-#pragma unroll
-        for (int ks = 0; ks < 4; ++ks)
-#pragma unroll
-            for (int r = 0; r < 4; ++r) {
-                float h, l;
-                split_tf32(x[ks][r], h, l);
-                ah[ks][r] = __float_as_uint(h); al[ks][r] = __float_as_uint(l);
-            }
-    };
     // consumer: the three products of one unit against the B tile at b_hi (B_lo 2 KB behind it), committed as one group; the
     // fragment registers stay read until the group retires
     auto mma_issue = [&](float (&acc)[8], float (&acc2)[8], const uint32_t (&ah)[4][4], const uint32_t (&al)[4][4], uint32_t b_hi) {
@@ -358,7 +333,9 @@ __global__ void __launch_bounds__(STC_THREADS, 1) sd_tc_kernel(const __grid_cons
     auto fetch = [&](Stage& g, bool transposed, uint32_t (&ah)[4][4], uint32_t (&al)[4][4]) {
         mbar_wait(smem_u32(&s_full[g.s]), g.sp);
         if (ct == 0) UTR(2);
-        load_frags(base + (size_t)g.s * STC_STAGE_BYTES, transposed, ah, al);
+        // this thread's A fragments of the unit, split into hi / lo (tc_ptx.cuh). Adjoint: [128 rows][32 k] with the 128-byte
+        // swizzle; apply: [32 k][128 rows] linear (512-byte lines)
+        load_frags_split(base + (size_t)g.s * STC_STAGE_BYTES, r0, kq, 0, transposed, ah, al);
         if (ct == 0) UTR(9);
         release(g);
         if (ct == 0) UTR(5);

@@ -1,6 +1,6 @@
 // PTX wrappers shared by the Hopper tensor-core kernels (conv_tc.cu, sd_tc.cu): mbarrier, TMA tensor loads, warpgroup MMAs
-// (wgmma.mma_async, TF32 in / FP32 accumulate in registers), the K-major SWIZZLE_128B shared-memory descriptor and the split used
-// for 3xTF32.
+// (wgmma.mma_async, TF32 in / FP32 accumulate in registers), the K-major SWIZZLE_128B shared-memory descriptor, the split used
+// for 3xTF32 and the register-A fragment load that applies it.
 #pragma once
 #include "common.cuh"
 #include <cuda.h>
@@ -95,13 +95,13 @@ __device__ __forceinline__ void wg_reg_fence(float (&d)[R]) {
     for (int i = 0; i < R; ++i) asm volatile("" : "+f"(d[i])::"memory");
 }
 // D[64 x N] += A[64 x 8] * B[N x 8]^T, TF32 operands, FP32 accumulators (fragment layout of the PTX ISA: register 4j + 2h + e of
-// thread t holds row 16 (t / 32) + (t % 32) / 4 + 8h, column 8j + 2 (t % 4) + e). _ss: A and B from shared memory; _rs: A from
-// registers (a[0..3] = rows r, r + 8 at column t % 4, then the same rows at column t % 4 + 4), B from shared memory.
-__device__ __forceinline__ void wgmma_ss_n64(float (&d)[32], uint64_t adesc, uint64_t bdesc) {
+// thread t holds row 16 (t / 32) + (t % 32) / 4 + 8h, column 8j + 2 (t % 4) + e), A from registers (a[0..3] = rows r, r + 8 at
+// column t % 4, then the same rows at column t % 4 + 4), B from shared memory; _ss: A from shared memory as well.
+__device__ __forceinline__ void wgmma_rs_n64(float (&d)[32], const uint32_t (&a)[4], uint64_t bdesc) {
     asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, 1, 0;\n\twgmma.mma_async.sync.aligned.m64n64k8.f32.tf32.tf32 "
-                 "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, %32, %33, p, 1, 1;\n\t}"
+                 "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, {%32, %33, %34, %35}, %36, p, 1, 1;\n\t}"
                  : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
-                 : "l"(adesc), "l"(bdesc) : "memory");
+                 : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(bdesc) : "memory");
 }
 
 __device__ __forceinline__ void wgmma_ss_n128(float (&d)[64], uint64_t adesc, uint64_t bdesc) {
@@ -116,6 +116,36 @@ __device__ __forceinline__ void wgmma_rs_n16(float (&d)[8], const uint32_t (&a)[
                  "{%0, %1, %2, %3, %4, %5, %6, %7}, {%8, %9, %10, %11}, %12, p, 1, 1;\n\t}"
                  : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7])
                  : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(bdesc) : "memory");
+}
+
+// byte offset of element (row, k) inside a K-major SWIZZLE_128B tile of 128-byte rows (tile base 1024-byte aligned)
+__device__ __forceinline__ uint32_t sw128(int row, int k) {
+    return (uint32_t)(row * 128 + ((((k >> 2) ^ (row & 7)) << 4) | ((k & 3) << 2)));
+}
+// One thread's register-A fragments of K steps ks0 .. ks0 + NKS - 1 (8 K columns x 4 registers each, the layout of the wgmma_rs_*
+// wrappers) of a 128 x 32 fp32 tile in shared memory, split into hi / lo: rows r0, r0 + 8 at K columns 8 ks + kq (+ 4), with
+// r0 = 64 (warpgroup) + 16 (warp % 4) + lane / 4 and kq = lane % 4. The tile is K-major with the 128-byte swizzle, or,
+// `transposed`, [32 k][128 rows] linear.
+template <int NKS>
+__device__ __forceinline__ void load_frags_split(const uint8_t* sb, int r0, int kq, int ks0, bool transposed, uint32_t (&ah)[NKS][4],
+                                                 uint32_t (&al)[NKS][4]) {
+    float x[NKS][4];
+#pragma unroll
+    for (int ks = 0; ks < NKS; ++ks) {
+#pragma unroll
+        for (int r = 0; r < 4; ++r) {
+            const int row = r0 + 8 * (r & 1), k = 8 * (ks0 + ks) + kq + 4 * (r >> 1);
+            x[ks][r] = transposed ? reinterpret_cast<const float*>(sb)[k * 128 + row] : *reinterpret_cast<const float*>(sb + sw128(row, k));
+        }
+    }
+#pragma unroll
+    for (int ks = 0; ks < NKS; ++ks)
+#pragma unroll
+        for (int r = 0; r < 4; ++r) {
+            float h, l;
+            split_tf32(x[ks][r], h, l);
+            ah[ks][r] = __float_as_uint(h); al[ks][r] = __float_as_uint(l);
+        }
 }
 
 // Host: fp32 tensor map (element strides 1, zero OOB fill) of rank 2..4, SWIZZLE_128B (box[0] = 32) or no swizzle; `strides_bytes`
