@@ -380,6 +380,16 @@ int b200trk_dimp_state_create(b200trk_dimp_state_t** out, b200trk_net_t* net, in
                               const float* label_lut, const float* mask_lut, const float* spatial_lut /* HOST [num_bins] */,
                               int num_bins, float bin_displacement, float feat_stride,
                               float step_length, float reg_weight, float alpha_eps);
+/* The same state with PrDiMPSteepestDescentNewton (ltr/models/target_classifier/optimizer.py:355-439) as its online optimiser, for
+ * PrDiMP: no LUTs; the hyper-parameters are the constructor arguments of that class, as b200trk_prdimp_sd_newton takes them
+ * (step_length = exp(log_step_length), reg_weight = max(filter_reg^2, min_filter_reg^2); has_softmax_reg == 0: softmax_reg = None).
+ * b200trk_dimp_update_host and the whole-frame calls then run the Newton update on the state's pitched sample memory. */
+int b200trk_prdimp_state_create(b200trk_dimp_state_t** out, b200trk_net_t* net, int memory_size, int filter_size,
+                                float gauss_sigma, float feat_stride, float step_length, float reg_weight, float alpha_eps,
+                                int has_softmax_reg, float softmax_reg, float label_threshold, int normalize_label,
+                                float label_shrink, float uni_weight);
+/* 0: DiMPSteepestDescentGN (b200trk_dimp_state_create), 1: PrDiMPSteepestDescentNewton (b200trk_prdimp_state_create). */
+int b200trk_dimp_state_optimizer_kind(b200trk_dimp_state_t* st);
 int b200trk_dimp_state_destroy(b200trk_dimp_state_t* st);
 /* Device views for the Python host (torch wraps them without copying): */
 float* b200trk_dimp_state_filter(b200trk_dimp_state_t* st);        /* [1,Cc,k,k]  */
@@ -476,6 +486,13 @@ typedef struct {
     int    box_refinement_relative;       /* box_refinement_space == 'relative' (PrDiMP) */
     int    update_scale_when_uncertain;   /* 1 */
     int    use_iounet_pos_for_learning;   /* 1 */
+    /* PrDiMP (pytracking/parameter/dimp/prdimp50.py); zero = the DiMP behaviour */
+    int    border_mode;                   /* sample_patch mode of the frame crops: 0 'replicate', 1 'inside', 2 'inside_major' (PrDiMP).
+                                             The native initial sample is always 'replicate' (see b200trk_dimp_tracker_init_state) */
+    double patch_max_scale_change;        /* 1.5 (PrDiMP); <= 0 = None (no upper bound on the shrink factor) */
+    int    score_preprocess;              /* localize_target's score pre-processing: 0 'none', 1 'exp', 2 'softmax' (PrDiMP) */
+    int    has_softmax_reg;               /* 1: softmax with the extra logit softmax_reg (the filter optimiser's softmax_reg) */
+    double softmax_reg;
 } b200trk_dimp_params_t;
 
 /* Crop request of one frame (sample_patch, preprocessing.py:55-148) -- what the crop kernel executes. */
@@ -497,8 +514,9 @@ typedef struct {
     int   scale_ind;
     int   r1, c1, r2, c2;     /* arg-max cell, and the second maximum outside the target neighbourhood (-1 when not computed) */
     int   use_second;         /* 1: the translation comes from (r2,c2) (dimp.py:291-292) */
-    float score1, score2;
-    float max_score;          /* torch.max(score_map) of the selected scale */
+    float score1, score2;     /* after score pre-processing (probabilities with score_preprocess = softmax) */
+    float max_score;          /* torch.max(score_map) of the selected scale after score pre-processing: the reference's
+                                 debug_info['max_score'] (dimp.py:153-159), i.e. the softmax probability for PrDiMP */
     int   pad_[6];
 } b200trk_loc_result_t;
 
@@ -588,7 +606,9 @@ int b200trk_dimp_tracker_state(const b200trk_dimp_tracker_t* t, float out[9]);
 int b200trk_sample_patch(const uint8_t* image_dev, int H, int W, const b200trk_crop_geom_t* geom, int win_h, int win_w, float* out,
                          b200trk_stream_t stream);
 /* localize_target / localize_advanced on the device: scores DEVICE [S,Ho,Wo]; neigh [S][2] = target_neigh_sz per scale,
- * prev_vec [S][2] = prev_target_vec per scale (HOST float32 arrays); result DEVICE b200trk_loc_result_t. */
+ * prev_vec [S][2] = prev_target_vec per scale (HOST float32 arrays); result DEVICE b200trk_loc_result_t. params->score_preprocess
+ * ('exp' / 'softmax' with params->softmax_reg, dimp.py:201-212) is applied per scale over the whole map before the arg-max; the
+ * raw scores are not modified. */
 int b200trk_dimp_localize(const float* scores, int S, int Ho, int Wo, const b200trk_dimp_params_t* params, const float* neigh,
                           const float* prev_vec, b200trk_loc_result_t* result_dev, b200trk_stream_t stream);
 

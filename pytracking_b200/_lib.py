@@ -56,7 +56,8 @@ class DimpParams(C.Structure):
                 ("box_jitter_sz", C.c_double), ("maximal_aspect_ratio", C.c_double), ("box_refinement_iter", C.c_int),
                 ("box_refinement_step_length", C.c_double), ("box_refinement_step_decay", C.c_double),
                 ("box_refinement_relative", C.c_int), ("update_scale_when_uncertain", C.c_int),
-                ("use_iounet_pos_for_learning", C.c_int)]
+                ("use_iounet_pos_for_learning", C.c_int), ("border_mode", C.c_int), ("patch_max_scale_change", C.c_double),
+                ("score_preprocess", C.c_int), ("has_softmax_reg", C.c_int), ("softmax_reg", C.c_double)]
 
 
 class CropGeom(C.Structure):
@@ -138,6 +139,8 @@ SIGNATURES = {
     "b200trk_prroi_pool_backward": (_I, [_VP, _VP, _VP, _VP, _VP, _I, _I, _I, _I, _I, _I, _I, _F, _VP]),
     "b200trk_prroi_pool_coor_backward": (_I, [_VP, _VP, _VP, _VP, _VP, _I, _I, _I, _I, _I, _I, _I, _F, _VP]),
     "b200trk_dimp_state_create": (_I, [C.POINTER(_VP), _VP, _I, _I, _VP, _VP, _VP, _I, _F, _F, _F, _F, _F]),
+    "b200trk_prdimp_state_create": (_I, [C.POINTER(_VP), _VP, _I, _I, _F, _F, _F, _F, _F, _I, _F, _F, _I, _F, _F]),
+    "b200trk_dimp_state_optimizer_kind": (_I, [_VP]),
     "b200trk_dimp_state_destroy": (_I, [_VP]),
     "b200trk_dimp_state_filter": (_VP, [_VP]),
     "b200trk_dimp_state_memory_pitch": (_I, [_VP]),

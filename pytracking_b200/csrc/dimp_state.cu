@@ -15,20 +15,13 @@ static int st_alloc(b200trk_dimp_state* s, void** p, size_t bytes) {
     return 0;
 }
 
-extern "C" int b200trk_dimp_state_create(b200trk_dimp_state_t** out, b200trk_net_t* net, int memory_size, int filter_size,
-                                         const float* label_lut, const float* mask_lut, const float* spatial_lut,
-                                         int num_bins, float bin_displacement, float feat_stride, float step_length,
-                                         float reg_weight, float alpha_eps) {
-    B200_REQUIRE(out && net && label_lut && mask_lut && spatial_lut, "dimp_state_create: null pointer");
-    B200_REQUIRE(memory_size >= 1 && memory_size <= 1024, "dimp_state_create: memory_size=%d", memory_size);
-    B200_REQUIRE(filter_size == 4, "dimp_state_create: filter_size=%d not supported (4)", filter_size);
-    B200_REQUIRE(num_bins >= 2 && num_bins <= 4096, "dimp_state_create: num_bins=%d", num_bins);
-    b200trk_dimp_state* s = new b200trk_dimp_state();
+// The buffers both optimiser kinds share (and the GN LUTs when num_bins > 0); frees `s` on failure.
+static int state_alloc(b200trk_dimp_state* s, b200trk_net* net, int memory_size, int filter_size, const float* label_lut,
+                       const float* mask_lut, const float* spatial_lut, int num_bins) {
     s->net = net; s->memory_size = memory_size; s->ksz = filter_size; s->max_batch = net->max_batch;
     s->Cc = net->dims[6]; s->Hc = net->dims[7]; s->Wc = net->dims[8];
     s->Ho = s->Hc + (filter_size + 1) % 2; s->Wo = s->Wc + (filter_size + 1) % 2;
-    s->num_bins = num_bins; s->bin_displacement = bin_displacement; s->feat_stride = feat_stride;
-    s->step_length = step_length; s->reg_weight = reg_weight; s->alpha_eps = alpha_eps;
+    s->num_bins = num_bins;
     const size_t plane = (size_t)s->Cc * s->Hc * s->Wc;
     int e = 0;
     if (!e) e = st_alloc(s, (void**)&s->filter, (size_t)s->Cc * 16 * sizeof(float));
@@ -41,8 +34,8 @@ extern "C" int b200trk_dimp_state_create(b200trk_dimp_state_t** out, b200trk_net
     if (!e) e = st_alloc(s, (void**)&s->crop, (size_t)s->max_batch * 3 * net->crop_h * net->crop_w * sizeof(float));
     if (!e) e = st_alloc(s, (void**)&s->maxval, (size_t)s->max_batch * sizeof(float));
     if (!e) e = st_alloc(s, (void**)&s->maxidx, (size_t)s->max_batch * 2 * sizeof(int64_t));
-    if (!e) e = st_alloc(s, (void**)&s->luts, (size_t)3 * num_bins * sizeof(float));
-    if (!e) {
+    if (!e && num_bins > 0) e = st_alloc(s, (void**)&s->luts, (size_t)3 * num_bins * sizeof(float));
+    if (!e && num_bins > 0) {
         cudaError_t ce = cudaMemcpy(s->luts, label_lut, num_bins * sizeof(float), cudaMemcpyHostToDevice);
         if (ce == cudaSuccess) ce = cudaMemcpy(s->luts + num_bins, mask_lut, num_bins * sizeof(float), cudaMemcpyHostToDevice);
         if (ce == cudaSuccess) ce = cudaMemcpy(s->luts + 2 * num_bins, spatial_lut, num_bins * sizeof(float), cudaMemcpyHostToDevice);
@@ -54,10 +47,48 @@ extern "C" int b200trk_dimp_state_create(b200trk_dimp_state_t** out, b200trk_net
             set_error("dimp_state_create: pinned staging allocation failed"); e = 1;
         }
     }
-    if (e) { b200trk_dimp_state_destroy(s); return e; }
+    if (e) b200trk_dimp_state_destroy(s);
+    return e;
+}
+
+extern "C" int b200trk_dimp_state_create(b200trk_dimp_state_t** out, b200trk_net_t* net, int memory_size, int filter_size,
+                                         const float* label_lut, const float* mask_lut, const float* spatial_lut,
+                                         int num_bins, float bin_displacement, float feat_stride, float step_length,
+                                         float reg_weight, float alpha_eps) {
+    B200_REQUIRE(out && net && label_lut && mask_lut && spatial_lut, "dimp_state_create: null pointer");
+    B200_REQUIRE(memory_size >= 1 && memory_size <= 1024, "dimp_state_create: memory_size=%d", memory_size);
+    B200_REQUIRE(filter_size == 4, "dimp_state_create: filter_size=%d not supported (4)", filter_size);
+    B200_REQUIRE(num_bins >= 2 && num_bins <= 4096, "dimp_state_create: num_bins=%d", num_bins);
+    b200trk_dimp_state* s = new b200trk_dimp_state();
+    s->opt_kind = b200trk_dimp_state::OPT_GN;
+    s->bin_displacement = bin_displacement; s->feat_stride = feat_stride;
+    s->step_length = step_length; s->reg_weight = reg_weight; s->alpha_eps = alpha_eps;
+    if (int e = state_alloc(s, net, memory_size, filter_size, label_lut, mask_lut, spatial_lut, num_bins)) return e;
     *out = s;
     return 0;
 }
+
+extern "C" int b200trk_prdimp_state_create(b200trk_dimp_state_t** out, b200trk_net_t* net, int memory_size, int filter_size,
+                                           float gauss_sigma, float feat_stride, float step_length, float reg_weight, float alpha_eps,
+                                           int has_softmax_reg, float softmax_reg, float label_threshold, int normalize_label,
+                                           float label_shrink, float uni_weight) {
+    B200_REQUIRE(out && net, "prdimp_state_create: null pointer");
+    B200_REQUIRE(memory_size >= 1 && memory_size <= 1024, "prdimp_state_create: memory_size=%d", memory_size);
+    B200_REQUIRE(filter_size == 4, "prdimp_state_create: filter_size=%d not supported (4)", filter_size);
+    B200_REQUIRE(gauss_sigma > 0.f && feat_stride > 0.f, "prdimp_state_create: gauss_sigma=%g and feat_stride=%g must be positive",
+                 gauss_sigma, feat_stride);
+    b200trk_dimp_state* s = new b200trk_dimp_state();
+    s->opt_kind = b200trk_dimp_state::OPT_NEWTON;
+    s->feat_stride = feat_stride; s->step_length = step_length; s->reg_weight = reg_weight; s->alpha_eps = alpha_eps;
+    s->gauss_sigma = gauss_sigma; s->has_softmax_reg = has_softmax_reg ? 1 : 0; s->softmax_reg = softmax_reg;
+    s->label_threshold = label_threshold; s->normalize_label = normalize_label ? 1 : 0; s->label_shrink = label_shrink;
+    s->uni_weight = uni_weight;
+    if (int e = state_alloc(s, net, memory_size, filter_size, nullptr, nullptr, nullptr, 0)) return e;
+    *out = s;
+    return 0;
+}
+
+extern "C" int b200trk_dimp_state_optimizer_kind(b200trk_dimp_state_t* s) { return s ? s->opt_kind : -1; }
 
 extern "C" int b200trk_dimp_state_destroy(b200trk_dimp_state_t* s) {
     if (!s) return 0;
@@ -115,13 +146,20 @@ int b200trk::dimp_state_update(b200trk_dimp_state* s, int scale_ind, int replace
     B200_CHECK_CUDA(cudaMemcpyAsync(s->boxes + 4 * replace_ind, h, 4 * sizeof(float), cudaMemcpyHostToDevice, st));
     B200_CHECK_CUDA(cudaMemcpyAsync(s->sw, h + 4, (size_t)n_stored * sizeof(float), cudaMemcpyHostToDevice, st));
     B200_CHECK_CUDA(cudaEventRecord(s->stage_ev[slot], st));
-    if (num_iter > 0) {
-        if (int e = dimp_sd_gn_pitched(s->filter, s->filter, s->memory, s->mem_pitch, s->boxes, s->sw, n_stored, s->Cc, s->Hc, s->Wc, s->ksz,
-                                       num_iter, s->luts, s->luts + s->num_bins, s->luts + 2 * s->num_bins, s->num_bins,
-                                       s->bin_displacement, s->feat_stride, s->step_length, s->reg_weight, s->alpha_eps,
-                                       nullptr, nullptr, st)) return e;
-    }
+    if (num_iter > 0) return dimp_state_optimize(s, n_stored, num_iter, st);
     return 0;
+}
+
+int b200trk::dimp_state_optimize(b200trk_dimp_state* s, int n_stored, int num_iter, cudaStream_t st) {
+    if (s->opt_kind == b200trk_dimp_state::OPT_NEWTON)
+        return prdimp_sd_newton_pitched(s->filter, s->filter, s->memory, s->mem_pitch, s->boxes, s->sw, n_stored, s->Cc, s->Hc, s->Wc, s->ksz,
+                                        num_iter, s->gauss_sigma, s->feat_stride, s->step_length, s->reg_weight, s->alpha_eps,
+                                        s->has_softmax_reg, s->softmax_reg, s->label_threshold, s->normalize_label, s->label_shrink,
+                                        s->uni_weight, nullptr, nullptr, st);
+    return dimp_sd_gn_pitched(s->filter, s->filter, s->memory, s->mem_pitch, s->boxes, s->sw, n_stored, s->Cc, s->Hc, s->Wc, s->ksz,
+                              num_iter, s->luts, s->luts + s->num_bins, s->luts + 2 * s->num_bins, s->num_bins,
+                              s->bin_displacement, s->feat_stride, s->step_length, s->reg_weight, s->alpha_eps,
+                              nullptr, nullptr, st);
 }
 
 extern "C" int b200trk_dimp_update_host(b200trk_dimp_state_t* s, int scale_ind, int replace_ind, const float* target_box_host,

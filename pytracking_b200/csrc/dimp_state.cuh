@@ -10,6 +10,12 @@ struct b200trk_dimp_state {
     int mem_pitch = 0;      // floats between two channel planes of the sample memory: H*W rounded up to 32, so that every 32-pixel
                             // TMA row of the optimiser is one 128-byte L2 line instead of straddling two
     float bin_displacement = 0.1f, feat_stride = 16.f, step_length = 1.f, reg_weight = 0.01f, alpha_eps = 0.f;
+    // which online optimiser updates the filter: DiMPSteepestDescentGN over the three LUTs (DiMP) or
+    // PrDiMPSteepestDescentNewton with the Gaussian-label hyper-parameters below (PrDiMP; no LUTs)
+    enum OptKind { OPT_GN = 0, OPT_NEWTON = 1 };
+    int opt_kind = OPT_GN;
+    float gauss_sigma = 0.f, softmax_reg = 0.f, label_threshold = 0.f, label_shrink = 0.f, uni_weight = 0.f;
+    int has_softmax_reg = 0, normalize_label = 0;
     float *filter = nullptr, *memory = nullptr, *boxes = nullptr, *sw = nullptr, *clf = nullptr, *scores = nullptr;
     float *crop = nullptr, *maxval = nullptr, *luts = nullptr;
     int64_t* maxidx = nullptr;
@@ -25,4 +31,6 @@ struct b200trk_dimp_state {
 namespace b200trk {
 int dimp_state_update(b200trk_dimp_state* s, int scale_ind, int replace_ind, const float* target_box_host,
                       const float* sample_weights_host, int n_stored, int num_iter, cudaStream_t st);
+// num_iter iterations of the state's online optimiser over the first n_stored samples of its pitched memory, filter in place
+int dimp_state_optimize(b200trk_dimp_state* s, int n_stored, int num_iter, cudaStream_t st);
 }

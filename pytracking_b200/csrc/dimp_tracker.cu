@@ -58,9 +58,34 @@ struct b200trk_dimp_tracker {
     b200trk_loc_result_t* loc_host = nullptr;      // pinned
 };
 
-// sample_patch geometry (preprocessing.py:55-148, mode 'replicate')
-static void plan_patch(const float pos[2], const float sample_sz[2], const float output_sz[2], int H, int W, b200trk_crop_geom_t* g) {
+// torch's floor division of float32 tensors (aten/src/ATen/native/BinaryOps.h div_floor_floating) for a divisor b > 0
+static float floor_div_f32(float a, float b) {
+    const float mod = std::fmod(a, b);
+    float div = (a - mod) / b;
+    if (mod != 0.f && (mod < 0.f)) div -= 1.0f;
+    if (div == 0.f) return std::copysign(0.f, a / b);
+    float fl = std::floor(div);
+    if (div - fl > 0.5f) fl += 1.0f;
+    return fl;
+}
+
+// sample_patch geometry (preprocessing.py:55-148). border_mode 0 'replicate'; 1 'inside' / 2 'inside_major' (preprocessing.py:76-86,
+// 112-122): the sample shrinks by the larger / smaller of its two size ratios to the image, clamped to [1, max_scale_change]
+// (max_scale_change <= 0: no upper bound), and is shifted inside the image -- or centred on it when it is larger. Padding stays
+// 'replicate' in every mode.
+static void plan_patch(const float pos[2], const float sample_sz_in[2], const float output_sz[2], int H, int W, int border_mode,
+                       double max_scale_change, b200trk_crop_geom_t* g) {
     long posl[2] = {(long)std::trunc(pos[0]), (long)std::trunc(pos[1])};                       // pos.long()
+    float sample_sz[2] = {sample_sz_in[0], sample_sz_in[1]};
+    const bool inside = border_mode == 1 || border_mode == 2;
+    if (inside) {
+        const float im_sz[2] = {(float)H, (float)W};                                           // torch.Tensor([H, W]): float32
+        const float s0 = sample_sz[0] / im_sz[0], s1 = sample_sz[1] / im_sz[1];
+        float shrink = border_mode == 1 ? std::fmax(s0, s1) : std::fmin(s0, s1);               // .max() / .min()
+        shrink = std::fmax(shrink, 1.0f);                                                      // clamp_(min=1, max=...)
+        if (max_scale_change > 0.0) shrink = std::fmin(shrink, f32(max_scale_change));
+        for (int i = 0; i < 2; ++i) sample_sz[i] = (float)(long)std::trunc(sample_sz[i] / shrink);   // (sample_sz / shrink).long()
+    }
     const float rf = std::fmin(sample_sz[0] / output_sz[0], sample_sz[1] / output_sz[1]);      // torch.min(sample_sz / output_sz).item()
     int df = (int)std::trunc((double)rf - 0.1);                                                // int(resize_factor - 0.1)
     if (df < 1) df = 1;
@@ -81,9 +106,19 @@ static void plan_patch(const float pos[2], const float sample_sz[2], const float
         const long szl = (long)std::fmax(std::nearbyint(sz[i]), 2.0f);                         // torch.max(sz.round(), 2).long()
         tl[i] = poslf[i] - ((float)(szl - 1) / 2.0f);                                          // posl - (szl - 1)/2
         br[i] = (poslf[i] + ((float)szl / 2.0f)) + 1.0f;                                       // posl + szl/2 + 1
-        tli[i] = (int)std::trunc(tl[i]); bri[i] = (int)std::trunc(br[i]);                      // .int().item()
     }
-    (void)H; (void)W;
+    if (inside) {
+        // im2_sz = the decimated image's size im[..., os::df, os::df]; tl, br stay float32 tensors throughout
+        const float im2[2] = {(float)((H - os[0] + df - 1) / df), (float)((W - os[1] + df - 1) / df)};
+        for (int i = 0; i < 2; ++i) {
+            const float shift = std::fmax(-tl[i], 0.0f) - std::fmax(br[i] - im2[i], 0.0f);     // (-tl).clamp(0) - (br - im2_sz).clamp(0)
+            tl[i] = tl[i] + shift; br[i] = br[i] + shift;
+            const float outside = floor_div_f32(std::fmax(-tl[i], 0.0f) + std::fmax(br[i] - im2[i], 0.0f), 2.0f);
+            const float shift2 = (-tl[i] - outside) * (outside > 0.0f ? 1.0f : 0.0f);          // (-tl - outside) * (outside > 0).long()
+            tl[i] = tl[i] + shift2; br[i] = br[i] + shift2;
+        }
+    }
+    for (int i = 0; i < 2; ++i) { tli[i] = (int)std::trunc(tl[i]); bri[i] = (int)std::trunc(br[i]); }   // .int().item()
     g->df = df; g->os_r = os[0]; g->os_c = os[1]; g->tl_r = tli[0]; g->tl_c = tli[1];
     g->in_h = bri[0] - tli[0]; g->in_w = bri[1] - tli[1];
     g->out_h = (int)output_sz[0]; g->out_w = (int)output_sz[1]; g->win_r = 0; g->win_c = 0;
@@ -112,6 +147,10 @@ static void iounet_box(const b200trk_dimp_tracker* t, const float pos[2], const 
 extern "C" int b200trk_dimp_tracker_create(b200trk_dimp_tracker_t** out, b200trk_dimp_state_t* state, const b200trk_dimp_params_t* params) {
     B200_REQUIRE(out && params, "dimp_tracker_create: null pointer");
     B200_REQUIRE(params->image_sample_size > 0 && params->sample_memory_size >= 1, "dimp_tracker_create: bad parameters");
+    B200_REQUIRE(params->border_mode >= 0 && params->border_mode <= 2, "dimp_tracker_create: border_mode=%d (0 replicate, 1 inside, 2 inside_major)",
+                 params->border_mode);
+    B200_REQUIRE(params->score_preprocess >= 0 && params->score_preprocess <= 2, "dimp_tracker_create: score_preprocess=%d (0 none, 1 exp, 2 softmax)",
+                 params->score_preprocess);
     B200_REQUIRE(!state || state->memory_size == params->sample_memory_size, "dimp_tracker_create: sample_memory_size=%d but the state holds %d",
                  params->sample_memory_size, state ? state->memory_size : 0);
     B200_REQUIRE(!state || (state->net->crop_h == params->image_sample_size && state->net->crop_w == params->image_sample_size),
@@ -156,6 +195,8 @@ extern "C" int b200trk_dimp_tracker_init_state(b200trk_dimp_tracker_t* t, int H,
                                                float init_target_box[4]) {
     B200_REQUIRE(t && b, "dimp_tracker_init_state: null pointer");
     B200_REQUIRE(H > 0 && W > 0 && b[2] > 0 && b[3] > 0, "dimp_tracker_init_state: bad image / box");
+    B200_REQUIRE(t->p.border_mode != 1, "dimp_tracker_init_state: border_mode 'inside' changes the initial sample (dimp.py:333-347), "
+                 "which the native initialisation does not implement; initialise with the reference and adopt its state");
     // dimp.py:44-76
     t->frame_num = 1;
     t->pos[0] = f32(b[1] + (b[3] - 1) / 2); t->pos[1] = f32(b[0] + (b[2] - 1) / 2);
@@ -182,7 +223,10 @@ extern "C" int b200trk_dimp_tracker_init_state(b200trk_dimp_tracker_t* t, int H,
     }
     const float sample_sz[2] = {init_scale * aug_sz[0], init_scale * aug_sz[1]};
     b200trk_crop_geom_t g;
-    plan_patch(init_pos, sample_sz, aug_sz, H, W, &g);
+    // Always border mode 'replicate' here: generate_init_samples (dimp.py:332-350) enters its border-mode block only for
+    // mode == 'inside', so 'inside_major' (PrDiMP) leaves the init crop alone, and sample_patch_transformed then samples with the
+    // default mode. 'inside' changes the init sample (scale and global shift); that is not implemented and refused above.
+    plan_patch(init_pos, sample_sz, aug_sz, H, W, 0, 0.0, &g);
     // Identity.crop_to_output (augmentation.py:20-37): pad by (output - image)/2, floor on the top / left side
     g.win_r = -(int)std::floor(((double)t->img_sample_sz[0] - (double)aug_sz[0]) / 2);
     g.win_c = -(int)std::floor(((double)t->img_sample_sz[1] - (double)aug_sz[1]) / 2);
@@ -232,7 +276,7 @@ extern "C" int b200trk_dimp_tracker_plan_crop(b200trk_dimp_tracker_t* t, b200trk
     }
     const float s = t->target_scale * 1.0f;                                                       // target_scale * scale_factors (ones(1))
     const float sample_sz[2] = {s * t->img_sample_sz[0], s * t->img_sample_sz[1]};
-    plan_patch(cpos, sample_sz, t->img_sample_sz, (int)t->image_sz[0], (int)t->image_sz[1], g);
+    plan_patch(cpos, sample_sz, t->img_sample_sz, (int)t->image_sz[0], (int)t->image_sz[1], t->p.border_mode, t->p.patch_max_scale_change, g);
     sample_location(t, g);
     return 0;
 }
@@ -487,8 +531,12 @@ extern "C" int b200trk_dimp_localize(const float* scores, int S, int Ho, int Wo,
     B200_REQUIRE(scores && p && result_dev, "dimp_localize: null pointer");
     B200_REQUIRE(S >= 1 && S <= 8 && Ho > 0 && Wo > 0, "dimp_localize: S=%d (1..8), map %dx%d", S, Ho, Wo);
     B200_REQUIRE(!p->advanced_localization || (neigh && prev_vec), "dimp_localize: advanced localisation needs neigh / prev_vec");
+    B200_REQUIRE(p->score_preprocess >= 0 && p->score_preprocess <= 2, "dimp_localize: score_preprocess=%d (0 none, 1 exp, 2 softmax)",
+                 p->score_preprocess);
     const LocArgs a = make_loc_args(S, Ho, Wo, p, neigh, prev_vec);
-    localize_kernel<<<1, 256, 0, (cudaStream_t)stream>>>(scores, a, result_dev);
+    const size_t smem = loc_smem_bytes(a);
+    B200_REQUIRE(smem <= 48 * 1024, "dimp_localize: score pre-processing holds S*Ho*Wo=%d floats in shared memory (at most 12288)", S * Ho * Wo);
+    localize_kernel<<<1, 256, smem, (cudaStream_t)stream>>>(scores, a, result_dev);
     B200_LAUNCH_CHECK();
     return 0;
 }
@@ -526,7 +574,9 @@ extern "C" int b200trk_dimp_tracker_initialize_host(b200trk_dimp_tracker_t* t, c
     const int iss = t->p.image_sample_size;
     if (int e = b200trk_sample_patch(t->img_dev, H, W, &g, iss, iss, s->crop, stream)) return e;
     if (int e = b200trk_net_forward(s->net, s->crop, 1, nullptr, nullptr, s->clf, stream)) return e;
-    // FilterInitializerZero (dimp.py:601-602) + net_opt_iter iterations on the single init sample (sample_weight = None -> 1/n)
+    // FilterInitializerZero (dimp.py:601-602) + net_opt_iter iterations on the single init sample. The reference passes
+    // sample_weight = None, which both optimisers read as 1/num_images (optimizer.py:122-123 GN, :387-388 Newton): with one sample
+    // that is the weight 1 uploaded here.
     B200_CHECK_CUDA(cudaMemsetAsync(s->filter, 0, (size_t)s->Cc * s->ksz * s->ksz * sizeof(float), st));
     B200_CHECK_CUDA(cudaMemsetAsync(s->sw, 0, (size_t)s->memory_size * sizeof(float), st));
     const float one = 1.f;
@@ -581,10 +631,7 @@ static int track_frame(b200trk_dimp_tracker* t, const uint8_t* image, bool on_de
         if (int e = dimp_state_update(s, 0, info->replace_ind, info->target_box, t->sw.data(), info->n_stored, info->num_iter, st)) return e;
     } else if (info->num_iter > 0) {
         // update_classifier can optimise without storing a sample (train_sample_interval > 1): run the iterations only
-        if (int e = dimp_sd_gn_pitched(s->filter, s->filter, s->memory, s->mem_pitch, s->boxes, s->sw, info->n_stored, s->Cc, s->Hc, s->Wc,
-                                       s->ksz, info->num_iter, s->luts, s->luts + s->num_bins, s->luts + 2 * s->num_bins, s->num_bins,
-                                       s->bin_displacement, s->feat_stride, s->step_length, s->reg_weight, s->alpha_eps, nullptr, nullptr, st))
-            return e;
+        if (int e = dimp_state_optimize(s, info->n_stored, info->num_iter, st)) return e;
     }
     return 0;
 }

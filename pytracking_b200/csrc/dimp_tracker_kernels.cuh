@@ -65,6 +65,8 @@ struct LocArgs {
     double not_found_thr, uncertain_thr, hard_sample_thr;
     float distractor_thr, hard_negative_thr, not_found_thr_f, disp_thr;
     float neigh[8][2], prev_vec[8][2];
+    int preprocess, has_reg;          // score_preprocess: 0 none, 1 exp, 2 softmax (with the extra logit `reg` when has_reg)
+    float reg;
 };
 
 struct AM { float v; int r, c; };
@@ -88,10 +90,73 @@ __device__ AM block_argmax(AM m, AM* red) {
     return r;
 }
 
-__global__ void __launch_bounds__(256) localize_kernel(const float* __restrict__ scores, LocArgs a, b200trk_loc_result_t* __restrict__ res) {
+// Block-wide max / sum in the order of softmax_reg_kernel (atom_ops_kernels.cuh) and block_sum (common.cuh): xor-shuffle within each
+// warp, then over the warp partials.
+__device__ __forceinline__ float loc_warp_max(float v) {
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) v = fmaxf(v, __shfl_xor_sync(0xffffffffu, v, o));
+    return v;
+}
+__device__ __forceinline__ float loc_warp_sum(float v) {
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
+    return v;
+}
+__device__ __forceinline__ float loc_block_max(float v, float* red) {
+    v = loc_warp_max(v);
+    __syncthreads();
+    if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = v;
+    __syncthreads();
+    float m = red[0];
+    for (int w = 1; w < (int)(blockDim.x + 31) / 32; ++w) m = fmaxf(m, red[w]);
+    return m;
+}
+__device__ __forceinline__ float loc_block_sum(float v, float* red) {
+    const int lane = threadIdx.x & 31;
+    v = loc_warp_sum(v);
+    __syncthreads();
+    if (lane == 0) red[threadIdx.x >> 5] = v;
+    __syncthreads();
+    const int nw = (blockDim.x + 31) >> 5;
+    return loc_warp_sum(lane < nw ? red[lane] : 0.f);
+}
+
+// Launch: dynamic shared memory of S * Ho * Wo floats when a.preprocess != 0 (loc_smem_bytes), none otherwise.
+#ifdef B200_CPU_EMUL
+#define B200_LOC_DYN_SMEM(name) float* name = reinterpret_cast<float*>(::cpu_emul::dyn_smem())
+#else
+#define B200_LOC_DYN_SMEM(name) extern __shared__ float name[]
+#endif
+__global__ void __launch_bounds__(256) localize_kernel(const float* __restrict__ scores_in, LocArgs a, b200trk_loc_result_t* __restrict__ res) {
     __shared__ AM red[8];
     const int n = a.Ho * a.Wo;
     const AM none = {__int_as_float(0xff800000), 1 << 30, 1 << 30};
+    // score_preprocess (dimp.py:201-212), per scale over the whole map (scores.view(S, -1)), into shared memory; everything below
+    // reads the pre-processed map. 'softmax' is activation.softmax_reg with the arithmetic of softmax_reg_kernel (atom_ops_kernels.cuh):
+    // m = max(reg, max x), p = expf(x - m) / (sum expf(x - m) + expf(reg - m)).
+    const float* scores = scores_in;
+    if (a.preprocess != 0) {
+        B200_LOC_DYN_SMEM(pre);
+        __shared__ float fred[32];
+        for (int s = 0; s < a.S; ++s) {
+            const float* x = scores_in + (size_t)s * n;
+            float* y = pre + (size_t)s * n;
+            if (a.preprocess == 1) {
+                for (int i = threadIdx.x; i < n; i += blockDim.x) y[i] = expf(x[i]);
+                continue;
+            }
+            float m = a.has_reg ? a.reg : __int_as_float(0xff800000);
+            for (int i = threadIdx.x; i < n; i += blockDim.x) m = fmaxf(m, x[i]);
+            m = loc_block_max(m, fred);
+            float e = 0.f;
+            for (int i = threadIdx.x; i < n; i += blockDim.x) e += expf(x[i] - m);
+            e = loc_block_sum(e, fred);
+            const float den = e + (a.has_reg ? expf(a.reg - m) : 0.f);
+            for (int i = threadIdx.x; i < n; i += blockDim.x) y[i] = __fdiv_rn(expf(x[i] - m), den);
+        }
+        __syncthreads();
+        scores = pre;
+    }
     // max_score1, max_disp1 per scale; scale_ind = first scale with the largest maximum (torch.max(max_score1, dim=0))
     AM best1 = none; int scale_ind = 0;
     for (int s = 0; s < a.S; ++s) {
@@ -161,7 +226,12 @@ inline LocArgs make_loc_args(int S, int Ho, int Wo, const b200trk_dimp_params_t*
             a.neigh[s][i] = (s < S && neigh) ? neigh[2 * s + i] : 0.f;
             a.prev_vec[s][i] = (s < S && prev_vec) ? prev_vec[2 * s + i] : 0.f;
         }
+    a.preprocess = p->score_preprocess; a.has_reg = p->has_softmax_reg ? 1 : 0;
+    a.reg = (float)p->softmax_reg;                  // x.new_tensor([reg]): float32 (activation.py:12-13)
     return a;
 }
+
+// dynamic shared memory of localize_kernel: the pre-processed maps
+inline size_t loc_smem_bytes(const LocArgs& a) { return a.preprocess ? (size_t)a.S * a.Ho * a.Wo * sizeof(float) : 0; }
 
 }  // namespace

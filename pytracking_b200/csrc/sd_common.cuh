@@ -57,4 +57,12 @@ int dimp_sd_gn_pitched(const float* weights, float* weights_out, const float* fe
                        int num_bins, float bin_displacement, float feat_stride, float step_length,
                        float reg_weight, float alpha_eps, float* iterates_out, float* losses_out, cudaStream_t st);
 
+// b200trk_prdimp_sd_newton with an explicit channel-plane pitch of the sample memory (0 = dense); used by dimp_state.cu
+int prdimp_sd_newton_pitched(const float* weights, float* weights_out, const float* feat, int feat_pitch, const float* bb,
+                             const float* sample_weight, int n, int C, int H, int W, int k, int num_iter,
+                             float gauss_sigma, float feat_stride, float step_length, float reg_weight,
+                             float alpha_eps, int has_softmax_reg, float softmax_reg, float label_threshold,
+                             int normalize_label, float label_shrink, float uni_weight,
+                             float* iterates_out, float* losses_out, cudaStream_t st);
+
 }  // namespace b200trk

@@ -141,19 +141,20 @@ extern "C" int b200trk_dimp_sd_gn(const float* weights, float* weights_out, cons
                               (cudaStream_t)stream);
 }
 
-extern "C" int b200trk_prdimp_sd_newton(const float* weights, float* weights_out, const float* feat, const float* bb,
-                                        const float* sample_weight, int n, int C, int H, int W, int k, int num_iter,
-                                        float gauss_sigma, float feat_stride, float step_length, float reg_weight,
-                                        float alpha_eps, int has_softmax_reg, float softmax_reg, float label_threshold,
-                                        int normalize_label, float label_shrink, float uni_weight,
-                                        float* iterates_out, float* losses_out, b200trk_stream_t stream) {
+int b200trk::prdimp_sd_newton_pitched(const float* weights, float* weights_out, const float* feat, int feat_pitch, const float* bb,
+                                      const float* sample_weight, int n, int C, int H, int W, int k, int num_iter,
+                                      float gauss_sigma, float feat_stride, float step_length, float reg_weight,
+                                      float alpha_eps, int has_softmax_reg, float softmax_reg, float label_threshold,
+                                      int normalize_label, float label_shrink, float uni_weight,
+                                      float* iterates_out, float* losses_out, cudaStream_t st) {
     if (int e = check_common("prdimp_sd_newton", weights, weights_out, feat, bb, n, C, H, W, k, num_iter)) return e;
     B200_REQUIRE(gauss_sigma > 0.f, "prdimp_sd_newton: gauss_sigma must be > 0 (one-hot labels not implemented)");
-    cudaStream_t st = (cudaStream_t)stream;
+    B200_REQUIRE(feat_pitch == 0 || (feat_pitch >= H * W && feat_pitch % 2 == 0), "prdimp_sd_newton: bad channel-plane pitch %d", feat_pitch);
     if (iterates_out)
         B200_CHECK_CUDA(cudaMemcpyAsync(iterates_out, weights, (size_t)C * 16 * sizeof(float), cudaMemcpyDeviceToDevice, st));
     SdParams P{};
     P.w_in = weights; P.w_out = weights_out; P.feat = feat; P.bb = bb; P.sample_weight = sample_weight;
+    P.feat_pitch = (feat_pitch == H * W) ? 0 : feat_pitch;
     P.n = n; P.C = C; P.num_iter = num_iter;
     P.gauss_sigma = gauss_sigma; P.has_softmax_reg = has_softmax_reg; P.softmax_reg = softmax_reg;
     P.label_threshold = label_threshold; P.normalize_label = normalize_label; P.label_shrink = label_shrink;
@@ -163,6 +164,17 @@ extern "C" int b200trk_prdimp_sd_newton(const float* weights, float* weights_out
     P.iterates_out = iterates_out; P.losses_out = losses_out;
     if (H == 18) return launch_sd<18, 1>(P, st);
     return launch_sd<22, 1>(P, st);
+}
+
+extern "C" int b200trk_prdimp_sd_newton(const float* weights, float* weights_out, const float* feat, const float* bb,
+                                        const float* sample_weight, int n, int C, int H, int W, int k, int num_iter,
+                                        float gauss_sigma, float feat_stride, float step_length, float reg_weight,
+                                        float alpha_eps, int has_softmax_reg, float softmax_reg, float label_threshold,
+                                        int normalize_label, float label_shrink, float uni_weight,
+                                        float* iterates_out, float* losses_out, b200trk_stream_t stream) {
+    return prdimp_sd_newton_pitched(weights, weights_out, feat, 0, bb, sample_weight, n, C, H, W, k, num_iter, gauss_sigma, feat_stride,
+                                    step_length, reg_weight, alpha_eps, has_softmax_reg, softmax_reg, label_threshold, normalize_label,
+                                    label_shrink, uni_weight, iterates_out, losses_out, (cudaStream_t)stream);
 }
 
 extern "C" int b200trk_dimp_l2_sd_gn(const float* weights, float* weights_out, const float* feat, const float* bb,

@@ -6,6 +6,7 @@ does on the host (pytracking/tracker/dimp/dimp.py): localisation decisions on th
 sample-weight bookkeeping; every tensor op runs in the CUDA library.
 """
 import ctypes as C
+import math
 
 import numpy as np
 import torch
@@ -73,23 +74,58 @@ class SampleWeights:
         return r_ind
 
 
+def newton_scalars(state_dict, nw):
+    """(step_length, reg_weight) of PrDiMPSteepestDescentNewton in float32, as its parameters give them: exp(log_step_length) and
+    (filter_reg^2).clamp(min=min_filter_reg^2) (optimizer.py:378-379).  log_step_length / filter_reg come from the state_dict when it
+    carries them (a trained net), else from the constructor arguments; params.filter_reg (nw['filter_reg_override']) replaces both
+    filter_reg and min_filter_reg, as DiMP._overwrite_classifier_params does (dimp.py:598-600)."""
+    po = "classifier.filter_optimizer."
+    one = torch.ones(1)
+    log_step = state_dict[po + "log_step_length"].float().cpu() if po + "log_step_length" in state_dict else \
+        math.log(nw["init_step_length"]) * one
+    if nw.get("filter_reg_override") is not None:
+        freg = nw["filter_reg_override"] * one
+    elif po + "filter_reg" in state_dict:
+        freg = state_dict[po + "filter_reg"].float().cpu()
+    else:
+        freg = nw["init_filter_reg"] * one
+    return float(torch.exp(log_step).item()), float((freg * freg).clamp(min=nw["min_filter_reg"] ** 2).item())
+
+
 class DiMPFrameEngine:
     def __init__(self, state_dict, arch="resnet50", filter_size=4, memory_size=50, max_batch=1, crop_size=288,
-                 precision=0, alpha_eps=0.0, min_filter_reg=1e-3, bin_displacement=0.1, feat_stride=16.0, device=None):
+                 precision=0, alpha_eps=0.0, min_filter_reg=1e-3, bin_displacement=0.1, feat_stride=16.0, device=None, newton=None):
+        """newton: None for DiMP (DiMPSteepestDescentGN over the three LUTs of the state_dict), or a dict of
+        PrDiMPSteepestDescentNewton constructor arguments (tracker.NEWTON_DEFAULTS names) for PrDiMP; the GN keys are then not read.
+        A state_dict that carries the optimiser's learnt log_step_length / filter_reg (a trained PrDiMP net) supplies those two."""
         self.backbone = BackboneEngine(state_dict, arch, filter_size, max_batch, crop_size, precision, device)
         self.device = self.backbone.device
         po = "classifier.filter_optimizer."
-        luts = [state_dict[po + k].detach().float().reshape(-1).contiguous().cpu() for k in
-                ("label_map_predictor.weight", "target_mask_predictor.0.weight", "spatial_weight_predictor.weight")]
-        self.step_length = float(torch.exp(state_dict[po + "log_step_length"].float()).item())
-        self.reg_weight = max(float(state_dict[po + "filter_reg"].float().item()) ** 2, min_filter_reg ** 2)
         self.memory_size, self.filter_size, self.max_batch = memory_size, filter_size, max_batch
+        self.newton = None
         h = C.c_void_p()
-        with torch.cuda.device(self.device):
-            _lib.check(_lib.lib().b200trk_dimp_state_create(
-                C.byref(h), self.backbone.handle, memory_size, filter_size, C.c_void_p(luts[0].data_ptr()),
-                C.c_void_p(luts[1].data_ptr()), C.c_void_p(luts[2].data_ptr()), luts[0].numel(), bin_displacement,
-                feat_stride, self.step_length, self.reg_weight, alpha_eps), "dimp_state_create")
+        if newton is None:
+            luts = [state_dict[po + k].detach().float().reshape(-1).contiguous().cpu() for k in
+                    ("label_map_predictor.weight", "target_mask_predictor.0.weight", "spatial_weight_predictor.weight")]
+            self.step_length = float(torch.exp(state_dict[po + "log_step_length"].float()).item())
+            self.reg_weight = max(float(state_dict[po + "filter_reg"].float().item()) ** 2, min_filter_reg ** 2)
+            with torch.cuda.device(self.device):
+                _lib.check(_lib.lib().b200trk_dimp_state_create(
+                    C.byref(h), self.backbone.handle, memory_size, filter_size, C.c_void_p(luts[0].data_ptr()),
+                    C.c_void_p(luts[1].data_ptr()), C.c_void_p(luts[2].data_ptr()), luts[0].numel(), bin_displacement,
+                    feat_stride, self.step_length, self.reg_weight, alpha_eps), "dimp_state_create")
+        else:
+            from .tracker import newton_hparams
+            nw = newton_hparams(newton)
+            self.step_length, self.reg_weight = newton_scalars(state_dict, nw)
+            self.newton = nw
+            sreg = nw["softmax_reg"]
+            with torch.cuda.device(self.device):
+                _lib.check(_lib.lib().b200trk_prdimp_state_create(
+                    C.byref(h), self.backbone.handle, memory_size, filter_size, float(nw["gauss_sigma"]), float(nw["feat_stride"]),
+                    self.step_length, self.reg_weight, float(nw["alpha_eps"]), int(sreg is not None), 0.0 if sreg is None else float(sreg),
+                    float(nw["label_threshold"]), int(bool(nw["normalize_label"])), float(nw["label_shrink"]),
+                    float(nw["init_uni_weight"] or 0.0)), "prdimp_state_create")
         self.state = h
         L = _lib.lib()
         cc, hc, wc = self.backbone.dims[6:9]

@@ -23,7 +23,38 @@ _DEFAULTS = dict(                                    # pytracking/parameter/dimp
     uncertain_threshold=-math.inf, hard_sample_threshold=-math.inf, target_inside_ratio=0.2, augmentation_expansion_factor=None,
     output_not_found_box=False, use_iou_net=True, iounet_k=5, num_init_random_boxes=0, box_jitter_pos=0.0, box_jitter_sz=0.0,
     maximal_aspect_ratio=6.0, box_refinement_iter=0, box_refinement_step_length=1.0, box_refinement_step_decay=1.0,
-    box_refinement_space="default", update_scale_when_uncertain=True, use_iounet_pos_for_learning=True)
+    box_refinement_space="default", update_scale_when_uncertain=True, use_iounet_pos_for_learning=True,
+    border_mode="replicate", patch_max_scale_change=None, score_preprocess="none", softmax_reg=None, score_filter_ksz=1,
+    low_score_opt_threshold=None)
+
+BORDER_MODES = {"replicate": 0, "inside": 1, "inside_major": 2}
+SCORE_PREPROCESS = {"none": 0, "exp": 1, "softmax": 2}
+
+# PrDiMPSteepestDescentNewton's constructor arguments (ltr/models/target_classifier/optimizer.py:312-314) with its defaults
+NEWTON_DEFAULTS = dict(feat_stride=16, init_step_length=1.0, init_filter_reg=1e-2, gauss_sigma=1.0, min_filter_reg=1e-3, alpha_eps=0.0,
+                       init_uni_weight=None, normalize_label=False, label_shrink=0, softmax_reg=None, label_threshold=0.0)
+# TrackerParams entries that DiMP._overwrite_classifier_params (dimp.py:589-603) writes into the filter optimiser
+_NEWTON_PARAM_OVERRIDES = ("filter_reg", "softmax_reg", "label_threshold", "label_shrink")
+
+
+def newton_hparams(newton, params_source=None, **param_overrides):
+    """The Newton optimiser's hyper-parameters (constructor names; `init_step_length` / `init_filter_reg` stand for the learnt
+    exp(log_step_length) / filter_reg) after the TrackerParams overrides of _overwrite_classifier_params: params.filter_reg sets both
+    filter_reg and min_filter_reg (and is recorded as `filter_reg_override`, which takes precedence over a learnt filter_reg in the
+    state_dict); softmax_reg, label_threshold and label_shrink replace the optimiser's own values."""
+    unknown = set(newton) - set(NEWTON_DEFAULTS) - {"filter_reg_override"}
+    if unknown:
+        raise ValueError("b200trk: unknown PrDiMPSteepestDescentNewton arguments %s" % sorted(unknown))
+    h = dict(NEWTON_DEFAULTS, **newton)
+    for k in _NEWTON_PARAM_OVERRIDES:
+        v = param_overrides.get(k, getattr(params_source, k, None) if params_source is not None else None)
+        if v is None:
+            continue
+        if k == "filter_reg":          # pred_module.filter_reg[0] = min_filter_reg = params.filter_reg, whatever the net had learnt
+            h["init_filter_reg"] = h["min_filter_reg"] = h["filter_reg_override"] = float(v)
+        else:
+            h[k] = v
+    return h
 
 
 def make_params(source=None, **overrides):
@@ -62,6 +93,19 @@ def make_params(source=None, **overrides):
     p.box_refinement_relative = int(vals["box_refinement_space"] == "relative")
     p.update_scale_when_uncertain = int(bool(vals["update_scale_when_uncertain"]))
     p.use_iounet_pos_for_learning = int(bool(vals["use_iounet_pos_for_learning"]))
+    if vals["border_mode"] not in BORDER_MODES:
+        raise NotImplementedError("b200trk: border_mode %r (supported: %s)" % (vals["border_mode"], ", ".join(BORDER_MODES)))
+    p.border_mode = BORDER_MODES[vals["border_mode"]]
+    p.patch_max_scale_change = 0.0 if vals["patch_max_scale_change"] is None else float(vals["patch_max_scale_change"])
+    if vals["score_preprocess"] not in SCORE_PREPROCESS:
+        raise NotImplementedError("b200trk: score_preprocess %r (supported: %s)" % (vals["score_preprocess"], ", ".join(SCORE_PREPROCESS)))
+    p.score_preprocess = SCORE_PREPROCESS[vals["score_preprocess"]]
+    p.has_softmax_reg = int(vals["softmax_reg"] is not None)
+    p.softmax_reg = 0.0 if vals["softmax_reg"] is None else float(vals["softmax_reg"])
+    if int(vals["score_filter_ksz"]) > 1:
+        raise NotImplementedError("b200trk: score_filter_ksz > 1 (a box filter on the score map) is not implemented")
+    if vals["low_score_opt_threshold"] is not None:
+        raise NotImplementedError("b200trk: low_score_opt_threshold (net_opt_low_iter schedule) is not implemented")
     return p
 
 
@@ -118,13 +162,21 @@ class HostLogic:
 
 
 class DiMPTracker(HostLogic):
-    """initialize / track on one GPU.  `state_dict`: the DiMP network's state_dict (reference key names)."""
+    """initialize / track on one GPU.  `state_dict`: the DiMP network's state_dict (reference key names).
+    `newton`: None for DiMP; for PrDiMP the PrDiMPSteepestDescentNewton constructor arguments (NEWTON_DEFAULTS names), to which
+    params.filter_reg / softmax_reg / label_threshold / label_shrink apply as in DiMP._overwrite_classifier_params.  The localisation's
+    softmax then uses the optimiser's softmax_reg, as localize_target does (dimp.py:207)."""
 
-    def __init__(self, state_dict, params=None, arch="resnet50", precision=0, device=None, **param_overrides):
+    def __init__(self, state_dict, params=None, arch="resnet50", precision=0, device=None, newton=None, **param_overrides):
         self.params = params if isinstance(params, _lib.DimpParams) else make_params(params, **param_overrides)
         p = self.params
+        if newton is not None:
+            src = None if isinstance(params, _lib.DimpParams) else params
+            newton = newton_hparams(newton, src, **param_overrides)
+            p.has_softmax_reg = int(newton["softmax_reg"] is not None)
+            p.softmax_reg = 0.0 if newton["softmax_reg"] is None else float(newton["softmax_reg"])
         self.engine = DiMPFrameEngine(state_dict, arch=arch, filter_size=4, memory_size=p.sample_memory_size, max_batch=1,
-                                      crop_size=p.image_sample_size, precision=precision, device=device)
+                                      crop_size=p.image_sample_size, precision=precision, device=device, newton=newton)
         self.device = self.engine.device
         h = C.c_void_p()
         with torch.cuda.device(self.device):
@@ -174,10 +226,32 @@ class DiMPTracker(HostLogic):
             _lib.check(_lib.lib().b200trk_dimp_tracker_attach_iounet(self.handle, self.iou.handle, C.c_void_p(m3.data_ptr()),
                                                                      C.c_void_p(m4.data_ptr())), "dimp_tracker_attach_iounet")
 
+    @staticmethod
+    def newton_from_reference(ref):
+        """PrDiMPSteepestDescentNewton hyper-parameters of a reference PrDiMP `DiMP` object (after its initialize(), i.e. with the
+        parameter overrides already written into the optimiser), in the constructor's names."""
+        fo = ref.net.classifier.filter_optimizer
+        return dict(feat_stride=fo.feat_stride, init_step_length=float(torch.exp(fo.log_step_length.detach().float()).item()),
+                    init_filter_reg=float(fo.filter_reg.detach().float().reshape(-1)[0].item()), gauss_sigma=fo.gauss_sigma,
+                    min_filter_reg=fo.min_filter_reg, alpha_eps=fo.alpha_eps, init_uni_weight=fo.uni_weight,
+                    normalize_label=fo.normalize_label, label_shrink=fo.label_shrink, softmax_reg=fo.softmax_reg,
+                    label_threshold=fo.label_threshold)
+
     def adopt_reference(self, ref, image_hw):
-        """Take over from a reference `DiMP` object after its `initialize()` (any augmentation / initialiser): scalars, sample
-        weights, sample memory, boxes and filter are copied into the engine; tracking continues natively."""
+        """Take over from a reference `DiMP` or PrDiMP `DiMP` object after its `initialize()` (any augmentation / initialiser):
+        scalars, sample weights, sample memory, boxes and filter are copied into the engine; tracking continues natively.  For PrDiMP
+        the engine must have been built with the Newton optimiser (`newton=DiMPTracker.newton_from_reference(ref)`)."""
         e = self.engine
+        is_newton = type(ref.net.classifier.filter_optimizer).__name__ == "PrDiMPSteepestDescentNewton"
+        if is_newton != (e.newton is not None):
+            raise RuntimeError("DiMPTracker.adopt_reference: the reference runs %s, this tracker's state %s" % (
+                type(ref.net.classifier.filter_optimizer).__name__, "PrDiMPSteepestDescentNewton" if e.newton else "DiMPSteepestDescentGN"))
+        if is_newton:
+            nw = self.newton_from_reference(ref)
+            mine = {k: e.newton[k] for k in nw}
+            if any(float(nw[k] or 0) != float(mine[k] or 0) for k in nw if k not in ("init_step_length", "init_filter_reg")) or \
+                    (nw["softmax_reg"] is None) != (mine["softmax_reg"] is None):
+                raise RuntimeError("DiMPTracker.adopt_reference: Newton hyper-parameters differ from the reference's: %s vs %s" % (mine, nw))
         n = int(min(int(ref.num_stored_samples[0]), self.params.sample_memory_size))
         e.memory[:n].copy_(ref.training_samples[0][:n].to(self.device))
         e.boxes[:n].copy_(ref.target_boxes[:n].to(self.device))
