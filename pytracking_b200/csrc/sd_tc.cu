@@ -6,8 +6,9 @@
 //       A = X_i[128 channels x 32 pixels]  (K-major straight from the [n, C, H*W] sample memory, TMA box, 128-byte swizzle)
 //       B = R_i^T[16 taps x 32 pixels]      (gathered from the residual map once per iteration, resident in shared memory)
 //   apply sweep     T_i[p, tap] = sum_c X_i[p, c] * F[c, tap] ;  s_i[y, x] = sum_tap T_i[(y, x) shifted by the tap, tap]   (A f)
-//       A = X_i[128 pixels x 32 channels]  (the SAME [n, C, H*W] memory: the TMA box is 32 channel rows x 128 pixels; TF32 wgmma
-//                                            wants K-major operands, so A is read transposed from shared memory into registers)
+//       A = X_i[128 pixels x 32 channels]  (the SAME [n, C, H*W] memory: four TMA boxes of 32 channel rows x 32 pixels, 128-byte
+//                                            swizzle; TF32 wgmma wants K-major operands, so A is read transposed from shared
+//                                            memory into registers, in a pixel-to-row order that makes those reads conflict-free)
 //       B = F^T[16 taps x 32 channels]      (the filter / gradient, resident in shared memory for the whole sweep)
 //
 // fp32 fidelity as in conv_tc.cu: every operand is split x = hi + lo (both TF32, round to nearest), three MMAs per K step
@@ -29,7 +30,8 @@
 // TMA; warps 0-7 (two consumer warpgroups, rows 0-63 / 64-127 of the tile) read their A fragments into registers, split them, free
 // the stage and issue 4 K steps x 3 products as register-A wgmmas against the 16-row B operand in shared memory. Two register sets
 // of fragments alternate: unit i+1 is loaded and split while unit i's MMAs are in flight, and the consumers only drain the MMAs
-// (wait_group 0) where the accumulators are read (end of a gradient chunk / an apply segment). The B tiles of both sweeps live in
+// (wait_group 0) where the accumulators are read (end of a gradient chunk / an apply segment). The two warpgroups take turns at
+// issuing their MMAs, so that one loads and splits while the other issues. The B tiles of both sweeps live in
 // one shared-memory region: R^T of every (sample, pixel block) pair of the CTA's adjoint range, built by all threads right after
 // the residual, then F^T of all channel blocks, built after the gradient exchange. The producer also issues the first units of
 // the NEXT sweep while the CTAs sit in the grid barrier. All 288 threads run the element-wise phases between the sweeps.
@@ -54,7 +56,7 @@ constexpr int STC_QL_MAX = 64;              // apply segments of one sample (<= 
 struct SdTcParams {
     SdParams p;
     CUtensorMap map_t;      // [n][C][H*W] as {pixel, channel, sample}: box 32 pixels x 128 channels, SWIZZLE_128B (adjoint sweep)
-    CUtensorMap map_a;      // the same memory: box 128 pixels x 32 channels, no swizzle (apply sweep)
+    CUtensorMap map_a;      // the same memory: box 32 pixels x 32 channels, SWIZZLE_128B (apply sweep: four boxes per unit)
     float* gpart; float* gfinal; float* gnpart; float* qslots; float* hpart; float* lossr; float* lossw;
     unsigned* barrier;
     int smax, nchk, kba, slice_max, ns;
@@ -65,6 +67,16 @@ __device__ __forceinline__ int part_lo(long long U, int G, int b) { return (int)
 __device__ __forceinline__ int part_owner(long long U, int G, int u) { return (int)((((long long)u + 1) * G - 1) / U); }
 
 __device__ __forceinline__ float tf32_lo(float x) { return tf32_rna(x - tf32_rna(x)); }
+// x = hi + lo with both parts TF32: bit for bit what split_tf32 (tc_ptx.cuh) gives for every input, NaN and infinity included, in 7
+// instructions instead of 9. cvt.rna.tf32.f32 of a value with bits u is (u + 0x1000) & 0xffffe000 when the value is finite and
+// u & 0xffffe000 when it is not. When x is finite, x - hi is finite or an infinity, whose masked bits the + 0x1000 leaves as they
+// are; when x is not, x - hi is NaN. So the finiteness test of x serves both roundings.
+__device__ __forceinline__ void split_tf32_bits(float x, uint32_t& hi, uint32_t& lo) {
+    const uint32_t a = (fabsf(x) < __int_as_float(0x7f800000)) ? 0x1000u : 0u;
+    hi = (__float_as_uint(x) + a) & 0xffffe000u;
+    const float r = __fsub_rn(x, __uint_as_float(hi));
+    lo = (__float_as_uint(r) + a) & 0xffffe000u;
+}
 __device__ __forceinline__ float warp_sum_xor(float v) {
 #pragma unroll
     for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
@@ -231,6 +243,11 @@ __global__ void __launch_bounds__(STC_THREADS, 1) sd_tc_kernel(const __grid_cons
     // consumer fragment coordinates (wgmma m64n16k8): rows r0, r0 + 8 of the tile, K column kq (+4), accumulator columns 8j + 2kq (+1)
     const int wg = warp >> 2;
     const int r0 = wg * 64 + (warp & 3) * 16 + (lane >> 2), kq = lane & 3;
+    // apply sweep: fragment row r0 holds tile pixel pr0 and row r0 + 8 pixel pr0 + 8. Inside a 32-pixel box, pixel bits 0-1 come
+    // from lane / 4, bit 2 from the warp, bit 3 from the row half and bit 4 from lane / 16; the 128-byte swizzle XORs bits 2-4 with
+    // the channel (kq, +4), so the 32 lanes of every fragment load hit 32 different banks. The rows of an MMA do not mix, so the
+    // order changes no value: the epilogue stores each row at its pixel.
+    const int pr0 = wg * 64 + (warp & 2) * 16 + (warp & 1) * 4 + ((lane >> 2) & 3) + (lane >> 4) * 16;
     const int ct = tid;                                               // consumer thread 0..255
 
     // F^T (hi | lo) of all channel blocks from a [C][16] vector in global memory
@@ -289,24 +306,26 @@ __global__ void __launch_bounds__(STC_THREADS, 1) sd_tc_kernel(const __grid_cons
     };
 
     // per-unit pipeline stamps (SM clock) of CTA 0 during the first adjoint sweep: utr[unit][16]
-    // 0 slot free (producer) 1 TMA issued | 2 tile landed (consumer) 9 operands in registers 5 stage released 7 MMAs committed
+    // producer: 0 slot free, 1 TMA issued | consumer thread 0: 2 tile landed, 9 operands in registers, 5 stage released, 8 the
+    // warpgroup's turn at the MMAs, 7 MMAs committed
     long long* utr = nullptr;
-    int utr_i = 0;
-#define UTR(k) do { if (utr && utr_i < 16) utr[utr_i * 16 + (k)] = clock64(); } while (0)
+#define UTR(u, k) do { if (utr && (unsigned)(u) < 16u) utr[(u) * 16 + (k)] = clock64(); } while (0)
     // ---- operand pipeline pieces --------------------------------------------------------------------------------------------
     // Every role walks the units of a sweep with RUNNING stage counters and unit coordinates (no integer division per unit).
     // ug = units since kernel start; shared-memory stage = ug % NS with parity (ug / NS) & 1.
     struct Stage { uint32_t s, sp; };
     auto stage_of = [&](uint32_t ug) { Stage g; g.s = ug % (uint32_t)NS; g.sp = (ug / (uint32_t)NS) & 1u; return g; };
     auto stage_next = [&](Stage& g) { if (++g.s == (uint32_t)NS) { g.s = 0; g.sp ^= 1u; } };
-    // producer: raw tile of one unit -> shared-memory stage g.s
-    auto produce = [&](const Stage& g, const CUtensorMap* map, int c0, int c1, int c2) {
+    // producer: raw tile of one unit -> shared-memory stage g.s as `nbox` boxes of `box_bytes`, the box origins 32 apart along c0;
+    // tu = the unit's row of the trace (-1: not traced)
+    auto produce = [&](const Stage& g, int tu, const CUtensorMap* map, int nbox, uint32_t box_bytes, int c0, int c1, int c2) {
         mbar_wait(smem_u32(&s_sfree[g.s]), g.sp ^ 1u);
-        if (lane == 0) UTR(0);
+        if (lane == 0) UTR(tu, 0);
         const uint32_t full = smem_u32(&s_full[g.s]);
-        mbar_expect_tx_elect(full, STC_STAGE_BYTES);
-        tma_load_3d_elect(base_u32 + g.s * STC_STAGE_BYTES, map, full, c0, c1, c2);
-        if (lane == 0) UTR(1);
+        mbar_expect_tx_elect(full, (uint32_t)nbox * box_bytes);
+        for (int q = 0; q < nbox; ++q)
+            tma_load_3d_elect(base_u32 + g.s * STC_STAGE_BYTES + (uint32_t)q * box_bytes, map, full, c0 + 32 * q, c1, c2);
+        if (lane == 0) UTR(tu, 1);
     };
     // consumer: the three products of one unit against the B tile at b_hi (B_lo 2 KB behind it), committed as one group; the
     // fragment registers stay read until the group retires
@@ -329,17 +348,46 @@ __global__ void __launch_bounds__(STC_THREADS, 1) sd_tc_kernel(const __grid_cons
         __syncwarp();
         if (lane == 0) mbar_arrive(smem_u32(&s_sfree[g.s]));
     };
-    // consumer: wait for the unit in stage g, take its fragments into registers, free the stage, advance g
-    auto fetch = [&](Stage& g, bool transposed, uint32_t (&ah)[4][4], uint32_t (&al)[4][4]) {
+    // consumer: wait for unit tu in stage g, take its fragments into registers, free the stage, advance g
+    auto fetch = [&](Stage& g, bool transposed, uint32_t (&ah)[4][4], uint32_t (&al)[4][4], int tu) {
         mbar_wait(smem_u32(&s_full[g.s]), g.sp);
-        if (ct == 0) UTR(2);
-        // this thread's A fragments of the unit, split into hi / lo (tc_ptx.cuh). Adjoint: [128 rows][32 k] with the 128-byte
-        // swizzle; apply: [32 k][128 rows] linear (512-byte lines)
-        load_frags_split(base + (size_t)g.s * STC_STAGE_BYTES, r0, kq, 0, transposed, ah, al);
-        if (ct == 0) UTR(9);
+        if (ct == 0) UTR(tu, 2);
+        // this thread's A fragments of the unit, split into hi / lo, in the register layout of wgmma_rs_n16: rows r, r + 8 at K
+        // columns 8 ks + kq (+ 4). Adjoint: [128 rows][32 k] with the 128-byte swizzle, r = r0; apply (`transposed`): four 32-pixel
+        // boxes [32 k][32 pixels] with the 128-byte swizzle, r = pr0
+        const uint8_t* sb = base + (size_t)g.s * STC_STAGE_BYTES;
+        float x[4][4];
+#pragma unroll
+        for (int ks = 0; ks < 4; ++ks)
+#pragma unroll
+            for (int r = 0; r < 4; ++r) {
+                const int row = (transposed ? pr0 : r0) + 8 * (r & 1), k = 8 * ks + kq + 4 * (r >> 1);
+                x[ks][r] = *reinterpret_cast<const float*>(sb + (transposed ? (row >> 5) * 4096 + sw128(k, row & 31) : sw128(row, k)));
+            }
+#pragma unroll
+        for (int ks = 0; ks < 4; ++ks)
+#pragma unroll
+            for (int r = 0; r < 4; ++r) split_tf32_bits(x[ks][r], ah[ks][r], al[ks][r]);
+        if (ct == 0) UTR(tu, 9);
         release(g);
-        if (ct == 0) UTR(5);
+        if (ct == 0) UTR(tu, 5);
         stage_next(g);
+    };
+    // The warpgroups take turns at the tensor cores, unit by unit: warpgroup 0 issues unit i, then warpgroup 1 issues unit i while
+    // warpgroup 0 loads and splits unit i+1, and so on. Issuing register-A MMAs keeps a warp busy about as long as the tensor cores
+    // take to run them, so the two must not issue at the same time and then load at the same time. Named barriers 2 (warpgroup 0's
+    // turn) and 3 (warpgroup 1's): each warpgroup waits for its own before unit i and hands the turn over after it; warpgroup 0
+    // needs no hand-over for the first unit and warpgroup 1 gives none after the last, so every sweep leaves both barriers clear.
+    // Both warpgroups walk the same units, so the turns never wait on a barrier the other warpgroup cannot reach.
+    auto turn_take = [&](int i) {
+        if (wg == 1) asm volatile("bar.sync 3, %0;" ::"n"(STC_CT) : "memory");
+        else if (i > 0) asm volatile("bar.sync 2, %0;" ::"n"(STC_CT) : "memory");
+        if (ct == 0) UTR(i, 8);
+    };
+    auto turn_pass = [&](int i, int nun) {
+        if (ct == 0) UTR(i, 7);
+        if (wg == 0) asm volatile("bar.arrive 3, %0;" ::"n"(STC_CT) : "memory");
+        else if (i + 1 < nun) asm volatile("bar.arrive 2, %0;" ::"n"(STC_CT) : "memory");
     };
 
     // unit coordinates: adjoint sweep (chunk, sample, pixel block), apply sweep (sample, pixel tile, channel block)
@@ -361,7 +409,8 @@ __global__ void __launch_bounds__(STC_THREADS, 1) sd_tc_kernel(const __grid_cons
         Stage g = stage_of(ug);
         AppPos c = app_pos(a_lo + i0);
         for (int i = i0; i < i1; ++i) {
-            produce(g, &Q.map_a, c.pt * 128, c.kb * 32, c.smp);
+            // the 32-pixel boxes that start inside the image (a box wholly past it would only feed rows the epilogue never reads)
+            produce(g, -1, &Q.map_a, min(4, (NPX - c.pt * 128 + 31) / 32), 4096u, c.pt * 128, c.kb * 32, c.smp);
             stage_next(g); app_next(c);
         }
     };
@@ -370,8 +419,7 @@ __global__ void __launch_bounds__(STC_THREADS, 1) sd_tc_kernel(const __grid_cons
         Stage g = stage_of(ug);
         AdjPos c = adj_pos(t_lo + i0);
         for (int i = i0; i < i1; ++i) {
-            if (traced) utr_i = i;
-            produce(g, &Q.map_t, c.kb * 32, c.chunk * 128, c.smp);
+            produce(g, traced ? i : -1, &Q.map_t, 1, (uint32_t)STC_STAGE_BYTES, c.kb * 32, c.chunk * 128, c.smp);
             stage_next(g); adj_next(c);
         }
     };
@@ -398,8 +446,10 @@ __global__ void __launch_bounds__(STC_THREADS, 1) sd_tc_kernel(const __grid_cons
                 auto step = [&](int i, const uint32_t (&ah)[4][4], const uint32_t (&al)[4][4], uint32_t (&nh)[4][4], uint32_t (&nl)[4][4]) {
                     const bool seg_first = (i == 0 || c.kb == 0), seg_last = (i == nun - 1 || c.kb == kba - 1);
                     if (seg_first) kb_first = c.kb;
+                    turn_take(i);
                     mma_issue(acc, acc2, ah, al, ftb_m + (uint32_t)c.kb * 4096u);
-                    if (i + 1 < nun) { wgmma_wait<1>(); fetch(g, true, nh, nl); }
+                    turn_pass(i, nun);
+                    if (i + 1 < nun) { wgmma_wait<1>(); fetch(g, true, nh, nl, i + 1); }
                     if (seg_last) {
                         mma_drain(acc, acc2);
                         // T[p][tap] of the finished segment: registers -> Tt[tap][p] -> shift-add over the taps -> qslots
@@ -410,7 +460,7 @@ __global__ void __launch_bounds__(STC_THREADS, 1) sd_tc_kernel(const __grid_cons
 #pragma unroll
                                 for (int e = 0; e < 2; ++e) {
                                     const int t = 4 * j + 2 * h + e;
-                                    Tt[(8 * j + 2 * kq + e) * STC_TT_PITCH + r0 + 8 * h] = acc2[t] + acc[t];
+                                    Tt[(8 * j + 2 * kq + e) * STC_TT_PITCH + pr0 + 8 * h] = acc2[t] + acc[t];
                                     acc[t] = 0.f; acc2[t] = 0.f;
                                 }
                         asm volatile("bar.sync 1, %0;" ::"n"(STC_CT) : "memory");
@@ -430,7 +480,7 @@ __global__ void __launch_bounds__(STC_THREADS, 1) sd_tc_kernel(const __grid_cons
                     }
                     app_next(c);
                 };
-                fetch(g, true, ah0, al0);
+                fetch(g, true, ah0, al0, 0);
                 for (int i = 0; i < nun; i += 2) {
                     step(i, ah0, al0, ah1, al1);
                     if (i + 1 < nun) step(i + 1, ah1, al1, ah0, al0);
@@ -464,10 +514,11 @@ __global__ void __launch_bounds__(STC_THREADS, 1) sd_tc_kernel(const __grid_cons
                 uint32_t ah0[4][4], al0[4][4], ah1[4][4], al1[4][4];
                 // as in the apply sweep: issue unit i, then load unit i+1 into the other register set once unit i-1 has retired
                 auto step = [&](int i, const uint32_t (&ah)[4][4], const uint32_t (&al)[4][4], uint32_t (&nh)[4][4], uint32_t (&nl)[4][4]) {
+                    turn_take(i);
                     mma_issue(acc, acc2, ah, al, rt_m + (uint32_t)sl * 4096u);
-                    if (ct == 0) UTR(7);
+                    turn_pass(i, nun);
                     if (++sl == per_chunk) sl = 0;
-                    if (i + 1 < nun) { wgmma_wait<1>(); utr_i = i + 1; fetch(g, false, nh, nl); }
+                    if (i + 1 < nun) { wgmma_wait<1>(); fetch(g, false, nh, nl, i + 1); }
                     if (--left == 0 || i == nun - 1) {
                         mma_drain(acc, acc2);
                         // the chunk's partial gradient: rows = channels of the chunk, columns = taps
@@ -484,8 +535,7 @@ __global__ void __launch_bounds__(STC_THREADS, 1) sd_tc_kernel(const __grid_cons
                         ++cl; left = per_chunk;
                     }
                 };
-                utr_i = 0;
-                fetch(g, false, ah0, al0);
+                fetch(g, false, ah0, al0, 0);
                 for (int i = 0; i < nun; i += 2) {
                     step(i, ah0, al0, ah1, al1);
                     if (i + 1 < nun) step(i + 1, ah1, al1, ah0, al0);
@@ -777,9 +827,9 @@ int launch_sd_tc(const SdParams& P0, cudaStream_t st, int* handled) {
         if ((pitch * 4) % 16 != 0) return 0;
         const uint64_t dims[3] = {(uint64_t)NPX, (uint64_t)C, (uint64_t)n};
         const uint64_t strides[2] = {pitch * 4, (uint64_t)C * pitch * 4};
-        const uint32_t box_t[3] = {32, 128, 1}, box_a[3] = {128, 32, 1};
+        const uint32_t box_t[3] = {32, 128, 1}, box_a[3] = {32, 32, 1};
         if (int e = tc_make_map(&Q.map_t, const_cast<float*>(P0.feat), 3, dims, strides, box_t, 1)) return e;
-        if (int e = tc_make_map(&Q.map_a, const_cast<float*>(P0.feat), 3, dims, strides, box_a, 0)) return e;
+        if (int e = tc_make_map(&Q.map_a, const_cast<float*>(P0.feat), 3, dims, strides, box_a, 1)) return e;
     }
 
     const size_t n_gpart = (size_t)G * STC_MAXCH * 128 * 16, n_q = (size_t)n * NPT * kba * NPOS;

@@ -47,12 +47,17 @@ print("call: %.1f us from the first stamp to the last iteration's residual" % ((
 u = np.array(list(ubuf), dtype=np.float64).reshape(16, 16)
 print("CTA 0, first adjoint sweep, per unit (SM clocks after the earliest stamp; '-' = not recorded: the producer issued the")
 print("first units during the previous sweep)")
-print("  producer: 0 slot free, 1 TMA issued | consumer thread 0: 2 tile landed, 9 operands in registers, 5 stage released, 7 MMAs committed")
+print("  producer: 0 slot free, 1 TMA issued | consumer thread 0: 2 tile landed, 9 operands in registers, 5 stage released,")
+print("  8 its warpgroup's turn at the MMAs came, 7 MMAs committed (the turn passes to the other warpgroup)")
 t00 = u[u > 0].min() if (u > 0).any() else 0
 for i in range(16):
     if u[i, 0] == 0 and u[i, 2] == 0:
         continue
-    print("  unit %2d: " % i + "  ".join(("%d:%7d" % (k, u[i, k] - t00)) if u[i, k] else ("%d:      -" % k) for k in (0, 1, 2, 9, 5, 7)))
+    print("  unit %2d: " % i + "  ".join(("%d:%7d" % (k, u[i, k] - t00)) if u[i, k] else ("%d:      -" % k) for k in (0, 1, 2, 9, 5, 8, 7)))
 d = np.diff(u[:, 2][u[:, 2] > 0])
 if len(d):
     print("  consumer period (tile landed -> next tile landed): median %d clocks" % np.median(d))
+for name, a, b in (("load + split (2 -> 9)", 2, 9), ("issue (8 -> 7)", 8, 7)):
+    ok = (u[:, a] > 0) & (u[:, b] > 0)
+    if ok.any():
+        print("  %s: median %d clocks" % (name, np.median(u[ok, b] - u[ok, a])))
