@@ -69,31 +69,6 @@ __device__ __forceinline__ unsigned ld_acquire_u32(const unsigned* p) {
     return v;
 }
 
-// Two-level grid barrier for COOPERATIVELY launched kernels: CTAs arrive on one of `fan` leaf counters (64-byte
-// apart, so the L2 atomics of different leaves do not serialise), the last arriver of a leaf arrives on the root, and
-// everybody polls the root.  `ctrs` = [root, pad.., leaf0 @ +16 words, leaf1 @ +32 words, ...], zeroed by the host
-// before launch; `epoch` counts barriers executed so far by this CTA (same on all CTAs).  All counters are monotonic.
-__device__ __forceinline__ void grid_barrier_tree(unsigned* ctrs, unsigned& epoch, int fan) {
-    __syncthreads();
-    epoch += 1;
-    if (threadIdx.x == 0) {
-        const int nb = gridDim.x;
-        const int leaf = blockIdx.x % fan;
-        const unsigned leaf_size = (unsigned)((nb - leaf + fan - 1) / fan);      // CTAs mapped to this leaf
-        __threadfence();
-        const unsigned prev = atomicAdd(ctrs + 16 * (leaf + 1), 1u);
-        if (prev + 1 == epoch * leaf_size) {        // last arriver of the leaf in this epoch
-            __threadfence();
-            atomicAdd(ctrs, 1u);
-        }
-        const unsigned nleaves = (unsigned)(nb < fan ? nb : fan);
-        const unsigned target = epoch * nleaves;
-        while (ld_acquire_u32(ctrs) < target) { }
-        __threadfence();
-    }
-    __syncthreads();
-}
-
 // Grid-wide barrier for COOPERATIVELY launched kernels (all CTAs co-resident). `counter` is zeroed by the
 // host before launch; `epoch` counts barriers executed so far by this CTA (same on all CTAs).
 __device__ __forceinline__ void grid_barrier(unsigned* counter, unsigned& epoch) {

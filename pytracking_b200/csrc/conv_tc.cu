@@ -56,7 +56,6 @@ struct TcParams {
     int relu;
     int cluster_red; // 1: the split-K CTAs of a tile form a thread-block cluster (1,1,splits) and reduce their partial tiles through
                      //    distributed shared memory instead of an L2 workspace + arrival counter
-    int prefetch_b;  // 1: the weight tiles of the first pipeline stages are requested before griddepcontrol.wait (they do not depend on the previous layer)
     uint32_t stage_bytes;
     uint32_t a_bytes, b_bytes;      // bytes one k-block's TMA lands: the A box | the B_hi and B_lo tiles
 };
@@ -154,7 +153,7 @@ __global__ void __launch_bounds__(TC_THREADS, 1) conv_tc_kernel(const __grid_con
     // The weights are constants: the producer requests the B tiles of the first stages now, so that only the activation tiles
     // remain to be fetched once the previous layer has completed.
     int npre = 0;
-    if (warp == 8 && P.prefetch_b) {
+    if (warp == 8) {
         npre = min(P.stages, nkb);
         int tap = kb0 / P.cblks, cb = kb0 - tap * P.cblks;
         for (int it = 0; it < npre; ++it) {
@@ -410,9 +409,7 @@ bool tc_conv_supported(const Op& op) {
     if (op.kind != OP_CONV) return false;
     if (!(op.k == 1 || op.k == 3)) return false;
     if (op.Cin % TC_KB != 0 || op.Cout % 64 != 0) return false;
-    if (op.stride == 2 && !env_int("B200TRK_TC_STRIDE2", 1)) return false;
-    if (op.stride != 1 && op.stride != 2) return false;
-    return env_int("B200TRK_TC", 1) != 0;
+    return op.stride == 1 || op.stride == 2;
 }
 
 int tc_make_map(CUtensorMap* m, float* base, int rank, const uint64_t* dims, const uint64_t* strides_bytes, const uint32_t* box,
@@ -543,7 +540,7 @@ static int tc_configure(b200trk_net* net, const Op& op, TcConv* tc, int S) {
         if (op.Cout % 128 == 0 && m_tiles * (op.Cout / 64) > net->sms) BN = 128;
         // long-K layers that still fill the SMs with 128-wide tiles through split-K (the DiMP head: 3x3, 1024 -> 512 at 18x18): the
         // K loop is bound by the operand bytes each CTA pulls from L2, and a wide tile re-reads the activations half as often
-        if (op.Cout % 128 == 0 && BN == 64 && env_int("B200TRK_TC_WIDE", 1)) {
+        if (op.Cout % 128 == 0 && BN == 64) {
             const int ctas128 = m_tiles * (op.Cout / 128);
             int sp = net->sms / (ctas128 > 0 ? ctas128 : 1);
             const int min_kb = env_int("B200TRK_TC_MINKB", 4);
@@ -578,7 +575,6 @@ static int tc_configure(b200trk_net* net, const Op& op, TcConv* tc, int S) {
     P.kb_per_split = (P.total_kb + splits - 1) / splits;
     P.splits = (P.total_kb + P.kb_per_split - 1) / P.kb_per_split;
     B200_REQUIRE(ctas <= 512 || P.splits == 1, "tc_conv: counter array too small for %d tiles", ctas);
-    P.ws = op.side ? net->splitk_ws2 : net->splitk_ws;
     P.cluster_red = (env_int("B200TRK_TC_CLUSTER", 1) && P.splits > 1 && P.splits <= 8) ? 1 : 0;
     if (P.cluster_red) {
         // Clusters that cannot all be resident at once reduce through the L2 workspace instead, as one wave of plain CTAs. Both
@@ -588,7 +584,6 @@ static int tc_configure(b200trk_net* net, const Op& op, TcConv* tc, int S) {
         if (int e = tc_max_active_clusters(P, ctas, &fit)) return e;
         if (fit < ctas) P.cluster_red = 0;
     }
-    P.prefetch_b = env_int("B200TRK_TC_PREFETCH_B", 1);
     // {K, Cout, hi | lo}: one box {32, BN, 2} lands B_hi and, BN * 128 bytes behind it, B_lo
     const uint64_t Kt = (uint64_t)op.k * op.k * op.Cin;
     const uint64_t bdims[3] = {Kt, (uint64_t)op.Cout, 2};
@@ -611,13 +606,9 @@ int tc_conv_launch(b200trk_net* net, const Op& op, int S, cudaStream_t st) {
     memset(&cfg, 0, sizeof(cfg));
     cfg.gridDim = grid; cfg.blockDim = dim3(TC_THREADS); cfg.dynamicSmemBytes = smem; cfg.stream = st;
     cudaLaunchAttribute at[2];
-    int nat = 0;
-    static const int use_pdl = env_int("B200TRK_TC_PDL", 1);
-    if (use_pdl) {
-        at[nat].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-        at[nat].val.programmaticStreamSerializationAllowed = 1;
-        ++nat;
-    }
+    at[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
+    at[0].val.programmaticStreamSerializationAllowed = 1;
+    int nat = 1;
     if (P.cluster_red) {
         at[nat].id = cudaLaunchAttributeClusterDimension;
         at[nat].val.clusterDim.x = 1; at[nat].val.clusterDim.y = 1; at[nat].val.clusterDim.z = (unsigned)P.splits;

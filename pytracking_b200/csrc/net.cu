@@ -4,7 +4,6 @@
 #include "net.cuh"
 #include <cmath>
 #include <cstring>
-#include <cstdlib>
 
 namespace b200trk {
 
@@ -142,27 +141,18 @@ static int build(b200trk_net* net, const b200trk_conv_desc_t* convs, int n_convs
             const int outp = bottleneck ? planes * 4 : planes;
             const bool has_ds = (bi == 0) && (stride != 1 || inplanes != outp);
             int c1, c2, c3, ds = -1, h1, w1, h2, w2, h3, w3;
-            const size_t i_c1 = net->ops.size();
-            size_t i_ds = 0;
             if (bottleneck) {
                 if (int e = B.add_conv(x, -1, H, W, inplanes, planes, 1, 1, 0, 1, &c1, &h1, &w1)) return e;
                 if (int e = B.add_conv(c1, -1, h1, w1, planes, planes, 3, stride, 1, 1, &c2, &h2, &w2)) return e;
                 // descriptor order = execution order: conv1, conv2, [downsample], conv3
-                i_ds = net->ops.size();
                 if (has_ds)
                     if (int e = B.add_conv(x, -1, H, W, inplanes, outp, 1, stride, 0, 0, &ds, &h3, &w3)) return e;
                 if (int e = B.add_conv(c2, has_ds ? ds : x, h2, w2, planes, outp, 1, 1, 0, 1, &c3, &h3, &w3)) return e;
             } else {
                 if (int e = B.add_conv(x, -1, H, W, inplanes, planes, 3, stride, 1, 1, &c1, &h1, &w1)) return e;
-                i_ds = net->ops.size();
                 if (has_ds)
                     if (int e = B.add_conv(x, -1, H, W, inplanes, outp, 1, stride, 0, 0, &ds, &h3, &w3)) return e;
                 if (int e = B.add_conv(c1, has_ds ? ds : x, h1, w1, planes, planes, 3, 1, 1, 1, &c3, &h3, &w3)) return e;
-            }
-            if (has_ds && net->n_forks < 4 && net->ops[i_ds].tc) {
-                // the shortcut convolution depends on the block input only: launched next to conv1 on the side stream (forward pass)
-                net->ops[i_c1].fork_op = (int)i_ds; net->ops[i_ds].side = 1; net->ops.back().join = 1;
-                net->ops[i_c1].ev = net->ops[i_ds].ev = net->ops.back().ev = net->n_forks++;
             }
             x = c3; H = h3; W = w3; inplanes = outp;
         }
@@ -213,16 +203,7 @@ extern "C" int b200trk_net_create(b200trk_net_t** out, int arch, const b200trk_c
     net->sms = device_sm_count();
     net->splitk_ws_floats = (size_t)8 << 20;   // 32 MB of split-K partials
     int e = dev_alloc(net, &net->splitk_ws, net->splitk_ws_floats);
-    if (!e) e = dev_alloc(net, &net->splitk_ws2, net->splitk_ws_floats);
     if (!e) e = build(net, convs, n_convs);
-    if (!e && net->n_forks > 0) {
-        cudaError_t ce = cudaStreamCreateWithFlags(&net->side_stream, cudaStreamNonBlocking);
-        for (int i = 0; i < net->n_forks && ce == cudaSuccess; ++i) {
-            ce = cudaEventCreateWithFlags(&net->ev_fork[i], cudaEventDisableTiming);
-            if (ce == cudaSuccess) ce = cudaEventCreateWithFlags(&net->ev_join[i], cudaEventDisableTiming);
-        }
-        if (ce != cudaSuccess) { set_error("net_create: side stream / events: %s", cudaGetErrorString(ce)); e = 1; }
-    }
     if (!e) e = dev_alloc(net, &net->l2_partials, 64 * 64);
     if (e) { b200trk_net_destroy(net); return e; }
     *out = net;
@@ -233,8 +214,6 @@ extern "C" int b200trk_net_destroy(b200trk_net_t* net) {
     if (!net) return 0;
     drop_graph(net);
     if (net->cap_stream) cudaStreamDestroy(net->cap_stream);
-    if (net->side_stream) cudaStreamDestroy(net->side_stream);
-    for (int i = 0; i < 4; ++i) { if (net->ev_fork[i]) cudaEventDestroy(net->ev_fork[i]); if (net->ev_join[i]) cudaEventDestroy(net->ev_join[i]); }
     for (auto& op : net->ops) if (op.tc) tc_conv_free(op.tc);
     for (void* p : net->owned) cudaFree(p);
     delete net;
@@ -379,10 +358,9 @@ extern "C" int b200trk_net_forward_iou(b200trk_net_t* net, const float* crop, in
     B200_REQUIRE((!iou3 && !iou4) || net->iou_dims[0] > 0, "net_forward: IoU features requested but no IoU head is attached");
     B200_REQUIRE(S >= 1 && S <= net->max_batch, "net_forward: batch %d outside [1,%d]", S, net->max_batch);
     cudaStream_t st = (cudaStream_t)stream;
-    static const bool use_graph = []() { const char* v = getenv("B200TRK_GRAPH"); return !v || atoi(v) != 0; }();
     cudaStreamCaptureStatus cs = cudaStreamCaptureStatusNone;
-    if (use_graph && cudaStreamIsCapturing(st, &cs) != cudaSuccess) { cudaGetLastError(); cs = cudaStreamCaptureStatusActive; }
-    if (!use_graph || cs != cudaStreamCaptureStatusNone) return net_forward_eager(net, crop, S, layer2, layer3, clf, iou3, iou4, st);
+    if (cudaStreamIsCapturing(st, &cs) != cudaSuccess) { cudaGetLastError(); cs = cudaStreamCaptureStatusActive; }
+    if (cs != cudaStreamCaptureStatusNone) return net_forward_eager(net, crop, S, layer2, layer3, clf, iou3, iou4, st);
     auto& k = net->gkey;
     const bool same = k.crop == crop && k.l2 == layer2 && k.l3 == layer3 && k.clf == clf && k.i3 == iou3 && k.i4 == iou4 && k.S == S;
     if (!same) {
@@ -419,23 +397,8 @@ extern "C" int b200trk_net_forward_iou(b200trk_net_t* net, const float* crop, in
 
 static int net_forward_eager(b200trk_net_t* net, const float* crop, int S, float* layer2, float* layer3, float* clf, float* iou3,
                              float* iou4, cudaStream_t st) {
-    // (off by default: measured 972 vs 974 frames/s with / without the fork on the DiMP-50 frame; B200TRK_NET_FORK=1 enables it)
-    static const bool fork_enabled = [] { const char* v = getenv("B200TRK_NET_FORK"); return v ? atoi(v) != 0 : false; }();
-    const bool fork = fork_enabled && net->side_stream != nullptr;
     for (const Op& op : net->ops) {
         if (op.iou && !iou3 && !iou4) continue;
-        if (fork && op.kind == OP_CONV) {
-            if (op.fork_op >= 0) {
-                // block input is complete at this point of `st`: start the shortcut convolution on the side stream
-                const Op& d = net->ops[op.fork_op];
-                B200_CHECK_CUDA(cudaEventRecord(net->ev_fork[d.ev], st));
-                B200_CHECK_CUDA(cudaStreamWaitEvent(net->side_stream, net->ev_fork[d.ev], 0));
-                if (int e = tc_conv_launch(net, d, S, net->side_stream)) return e;
-                B200_CHECK_CUDA(cudaEventRecord(net->ev_join[d.ev], net->side_stream));
-            }
-            if (op.side) continue;                    // launched at its block's fork point
-            if (op.join) B200_CHECK_CUDA(cudaStreamWaitEvent(st, net->ev_join[op.ev], 0));
-        }
         switch (op.kind) {
         case OP_PREPROCESS:
             if (int e = launch_preprocess(crop, net->bufs[op.out], S, op.Hin, op.Win, st)) return e;

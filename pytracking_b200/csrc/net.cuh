@@ -20,10 +20,6 @@ struct Op {
     int export_slot = -1;    // OP_EXPORT_NCHW: 0 = layer2, 1 = layer3, 2 / 3 = the IoUNet features of layer2 / layer3
     int iou = 0;             // belongs to the IoUNet feature branch (skipped when no IoU output is requested)
     TcConv* tc = nullptr;
-    // fork / join of a residual block's downsample conv (it only depends on the block input, so it runs on a side stream next to
-    // conv1 / conv2): `fork_op` (on conv1) = plan index of the downsample conv, `side` marks that conv, `join` (on the conv that
-    // adds the shortcut) waits for it; `ev` = event pair of the block
-    int fork_op = -1, side = 0, join = 0, ev = -1;
 };
 
 }  // namespace b200trk
@@ -36,10 +32,6 @@ struct b200trk_net {
     std::vector<size_t> buf_floats;      // per-sample floats of each buffer
     std::vector<void*> owned;            // every device allocation (freed in destroy)
     float* splitk_ws = nullptr; size_t splitk_ws_floats = 0;
-    float* splitk_ws2 = nullptr;         // split-K partials of the side-stream convolutions (they overlap main-stream ones)
-    cudaStream_t side_stream = nullptr;
-    cudaEvent_t ev_fork[4] = {nullptr, nullptr, nullptr, nullptr}, ev_join[4] = {nullptr, nullptr, nullptr, nullptr};
-    int n_forks = 0;
     float* l2_partials = nullptr;
     int dims[9] = {0};
     int feat_buf[2] = {-1, -1}, feat_hw[2][3] = {{0, 0, 0}, {0, 0, 0}};   // NHWC buffers / (C,H,W) of layer2 and layer3

@@ -46,11 +46,9 @@ static int launch_sd(SdParams P, cudaStream_t st) {
     const int sms = device_sm_count();
     const size_t limit = 227 * 1024 - 512;
     const size_t item = (size_t)K::ITEM_FLOATS * sizeof(float);
-    const int forced = [] { const char* v = getenv("B200TRK_SD_PASSES"); return v ? atoi(v) : 0; }();
     int passes = 0, NCH = 0, NG = 0, spc = 0, best_cost = 1 << 30;
     for (int p = 64; p >= 1; p >>= 1) {
         if (P.C % (SLOTS * p) != 0) continue;
-        if (forced && p != forced) continue;
         const int nch = P.C / (SLOTS * p);
         if (nch > sms) continue;
         int ng = sms / nch; if (ng > P.n) ng = P.n; if (ng < 1) ng = 1;

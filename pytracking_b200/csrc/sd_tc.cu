@@ -403,7 +403,6 @@ __global__ void __launch_bounds__(STC_THREADS, 1) sd_tc_kernel(const __grid_cons
     // shared-memory stages); those tiles land while the CTAs sit in the grid barriers / reductions between the sweeps.
     // pf_apply / pf_adj = units of the coming apply / adjoint sweep already issued.
     int pf_apply = 0, pf_adj = 0;
-    const bool xpf = true;
     auto produce_apply_run = [&](uint32_t ug, int i0, int i1) {        // units i0 .. i1-1 of this CTA's apply range; ug = global index of i0
         if (i0 >= i1) return;
         Stage g = stage_of(ug);
@@ -431,7 +430,7 @@ __global__ void __launch_bounds__(STC_THREADS, 1) sd_tc_kernel(const __grid_cons
             if (warp == 8) {
                 // (whole warp, converged: see tc_ptx.cuh)
                 produce_apply_run(ucount + (uint32_t)pf_apply, pf_apply, nun);
-                if (xpf && adjoint_follows) produce_adj_run(ucount + (uint32_t)nun, 0, min(NS, t_hi - t_lo), false);
+                if (adjoint_follows) produce_adj_run(ucount + (uint32_t)nun, 0, min(NS, t_hi - t_lo), false);
             } else {
                 const uint32_t ftb_m = smem_u32(ftb);
                 int kb_first = 0;
@@ -490,7 +489,7 @@ __global__ void __launch_bounds__(STC_THREADS, 1) sd_tc_kernel(const __grid_cons
         }
         ucount += (uint32_t)nun;
         pf_apply = 0;
-        pf_adj = (xpf && adjoint_follows && nun > 0) ? min(NS, t_hi - t_lo) : 0;
+        pf_adj = (adjoint_follows && nun > 0) ? min(NS, t_hi - t_lo) : 0;
         __syncthreads();
     };
 
@@ -502,7 +501,7 @@ __global__ void __launch_bounds__(STC_THREADS, 1) sd_tc_kernel(const __grid_cons
             const int chunk0 = t_lo / per_chunk;
             if (warp == 8) {
                 produce_adj_run(ucount + (uint32_t)pf_adj, pf_adj, nun, true);
-                if (xpf) produce_apply_run(ucount + (uint32_t)nun, 0, min(NS, a_hi - a_lo));   // an apply sweep always follows an adjoint sweep
+                produce_apply_run(ucount + (uint32_t)nun, 0, min(NS, a_hi - a_lo));   // an apply sweep always follows an adjoint sweep
             } else {
                 const uint32_t rt_m = smem_u32(ftb);
                 Stage g = stage_of(ucount);
@@ -545,7 +544,7 @@ __global__ void __launch_bounds__(STC_THREADS, 1) sd_tc_kernel(const __grid_cons
         }
         ucount += (uint32_t)nun;
         pf_adj = 0;
-        pf_apply = (xpf && nun > 0) ? min(NS, a_hi - a_lo) : 0;
+        pf_apply = (nun > 0) ? min(NS, a_hi - a_lo) : 0;
         __syncthreads();
     };
 

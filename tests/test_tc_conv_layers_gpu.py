@@ -17,9 +17,6 @@ Where e / e_tf32 is largest: the 3x3 1024 -> 512 classification head launched wi
 where one fp32 accumulator chain runs over all K = 9216 products; its fp32 summation error grows with the chain while e_tf32 shrinks
 as 1 / sqrt(K). Measured on an H100 80GB HBM3 (700 W): 0.057 there, at most 0.012 on every other plan's worst layer."""
 import ctypes as C
-import os
-import subprocess
-import sys
 
 import pytest
 import torch
@@ -30,7 +27,6 @@ from pytracking_b200.engine import BackboneEngine
 
 pytestmark = pytest.mark.gpu
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 OP_CONV, OP_L2NORM = 3, 5
 TINY = 1e-30
 
@@ -230,7 +226,7 @@ CASES = {
     "minkb1": dict(R288, env={"B200TRK_TC_MINKB": "1"}, reach=_reaches_uneven_split, repeat=True),
     "bn64": dict(R288, env={"B200TRK_TC_BN": "64"}, reach=_all_bn(64)),
     "bn128": dict(R288, env={"B200TRK_TC_BN": "128"}, reach=_all_bn(128)),
-    "noprefetch_nosplitk": dict(R288, env={"B200TRK_TC_PREFETCH_B": "0", "B200TRK_TC_SPLITK": "0"}, reach=_no_splitk),
+    "nosplitk": dict(R288, env={"B200TRK_TC_SPLITK": "0"}, reach=_no_splitk),
 }
 
 
@@ -266,19 +262,6 @@ def _run_case(name, setenv):
 @pytest.mark.parametrize("name", sorted(CASES))
 def test_tc_conv_layers_vs_float64(name, monkeypatch):
     _run_case(name, monkeypatch.setenv)
-
-
-def test_tc_conv_layers_side_stream_eager():
-    """B200TRK_NET_FORK and B200TRK_GRAPH are read once per process: the shortcut convolutions on the side stream (with their own
-    split-K workspace, reached through the L2 workspace plan) and eager launches run in a process of their own."""
-    env = dict(os.environ, B200TRK_NET_FORK="1", B200TRK_GRAPH="0")
-    code = ("import sys; sys.path[:0] = [%r, %r]; import test_tc_conv_layers_gpu as t, os; "
-            "t._run_case('r50_288_s1_iou', os.environ.__setitem__); t._run_case('cluster0', os.environ.__setitem__)"
-            % (ROOT, os.path.join(ROOT, "tests")))
-    flags = ["-s"] if sys.flags.no_user_site else []
-    p = subprocess.run([sys.executable] + flags + ["-c", code], cwd=ROOT, env=env, capture_output=True, text=True, timeout=1200)
-    print(p.stdout[-4000:])
-    assert p.returncode == 0, p.stderr[-4000:]
 
 
 def test_tc_conv_batch_size_switch_on_one_handle():
