@@ -612,6 +612,50 @@ int b200trk_sample_patch(const uint8_t* image_dev, int H, int W, const b200trk_c
 int b200trk_dimp_localize(const float* scores, int S, int Ho, int Wo, const b200trk_dimp_params_t* params, const float* neigh,
                           const float* prev_vec, b200trk_loc_result_t* result_dev, b200trk_stream_t stream);
 
+/* ------------------------------------------------------------------------------------------------
+ * A batch of sequences tracked in lock-step on one GPU: S slots (1..16), each a whole-frame tracker with its own online model
+ * (sample memory, boxes, weights, filter) on ONE network built for batches of S. A step takes one frame for any subset of the
+ * slots and runs one crop launch, one network forward at batch S (always S, whichever slots are busy: a sequence's results then
+ * depend only on its own frames and on S), one classify launch with each slot's filter, one localisation launch over the tracked
+ * slots, one 64-byte-per-slot read-back and one synchronisation; then each slot's host half (commit_localize / commit_update) and
+ * its memory insert + steepest-descent update, enqueued back to back on `stream`. use_iou_net is not supported.
+ * ---------------------------------------------------------------------------------------------- */
+typedef struct b200trk_dimp_batch b200trk_dimp_batch_t;
+
+/* One frame of one slot. init = 1 starts a (new) sequence in the slot with init_bbox (x, y, w, h): DiMP.initialize as
+ * b200trk_dimp_tracker_initialize_host runs it; init = 0 tracks the slot's running sequence (same frame size as its first frame). */
+typedef struct {
+    int            slot;
+    const uint8_t* image;         /* uint8 [H,W,3] RGB: HOST for step_host, DEVICE for step_device */
+    int            H, W;
+    int            init;
+    double         init_bbox[4];
+} b200trk_batch_item_t;
+
+/* DiMP (the GN optimiser's LUT arguments of b200trk_dimp_state_create) or PrDiMP (the Newton arguments of
+ * b200trk_prdimp_state_create); params are shared by every slot. `net` must have max_batch >= capacity and outlive the batch. */
+int b200trk_dimp_batch_create(b200trk_dimp_batch_t** out, b200trk_net_t* net, int capacity, const b200trk_dimp_params_t* params,
+                              int filter_size, const float* label_lut, const float* mask_lut, const float* spatial_lut, int num_bins,
+                              float bin_displacement, float feat_stride, float step_length, float reg_weight, float alpha_eps);
+int b200trk_prdimp_batch_create(b200trk_dimp_batch_t** out, b200trk_net_t* net, int capacity, const b200trk_dimp_params_t* params,
+                                int filter_size, float gauss_sigma, float feat_stride, float step_length, float reg_weight, float alpha_eps,
+                                int has_softmax_reg, float softmax_reg, float label_threshold, int normalize_label, float label_shrink,
+                                float uni_weight);
+int b200trk_dimp_batch_destroy(b200trk_dimp_batch_t* b);
+/* End the slot's sequence; the slot can be tracked again only after an init item. */
+int b200trk_dimp_batch_release(b200trk_dimp_batch_t* b, int slot);
+/* One step over n items (distinct slots); infos[n] receives what each item's frame did (for an init item: bbox = init_bbox). */
+int b200trk_dimp_batch_step_host(b200trk_dimp_batch_t* b, const b200trk_batch_item_t* items, int n, b200trk_frame_info_t* infos,
+                                 b200trk_stream_t stream);
+int b200trk_dimp_batch_step_device(b200trk_dimp_batch_t* b, const b200trk_batch_item_t* items, int n, b200trk_frame_info_t* infos,
+                                   b200trk_stream_t stream);
+/* Read-only DEVICE views of one slot (NULL for a bad slot): filter [C,k,k], the last step's scores [Ho,Wo] and crop [3,iss,iss];
+ * and the slot's scalar state as b200trk_dimp_tracker_state gives it. */
+float* b200trk_dimp_batch_filter(b200trk_dimp_batch_t* b, int slot);
+float* b200trk_dimp_batch_scores(b200trk_dimp_batch_t* b, int slot);
+float* b200trk_dimp_batch_crop(b200trk_dimp_batch_t* b, int slot);
+int b200trk_dimp_batch_state(const b200trk_dimp_batch_t* b, int slot, float out[9]);
+
 #ifdef __cplusplus
 }
 #endif

@@ -79,6 +79,11 @@ class FrameInfo(C.Structure):
                 ("loc", LocResult), ("crop", CropGeom), ("refined", C.c_int), ("predicted_iou", C.c_float)]
 
 
+class BatchItem(C.Structure):
+    """b200trk_batch_item_t"""
+    _fields_ = [("slot", C.c_int), ("image", C.c_void_p), ("H", C.c_int), ("W", C.c_int), ("init", C.c_int), ("init_bbox", C.c_double * 4)]
+
+
 # name -> (restype, argtypes); every symbol of include/b200trk.h is listed (tests check the export table against it)
 _VP, _I, _F = C.c_void_p, C.c_int, C.c_float
 SIGNATURES = {
@@ -174,6 +179,16 @@ SIGNATURES = {
     "b200trk_dimp_tracker_state": (_I, [_VP, C.POINTER(C.c_float * 9)]),
     "b200trk_sample_patch": (_I, [_VP, _I, _I, C.POINTER(CropGeom), _I, _I, _VP, _VP]),
     "b200trk_dimp_localize": (_I, [_VP, _I, _I, _I, C.POINTER(DimpParams), _VP, _VP, _VP, _VP]),
+    "b200trk_dimp_batch_create": (_I, [C.POINTER(_VP), _VP, _I, C.POINTER(DimpParams), _I, _VP, _VP, _VP, _I, _F, _F, _F, _F, _F]),
+    "b200trk_prdimp_batch_create": (_I, [C.POINTER(_VP), _VP, _I, C.POINTER(DimpParams), _I, _F, _F, _F, _F, _F, _I, _F, _F, _I, _F, _F]),
+    "b200trk_dimp_batch_destroy": (_I, [_VP]),
+    "b200trk_dimp_batch_release": (_I, [_VP, _I]),
+    "b200trk_dimp_batch_step_host": (_I, [_VP, C.POINTER(BatchItem), _I, C.POINTER(FrameInfo), _VP]),
+    "b200trk_dimp_batch_step_device": (_I, [_VP, C.POINTER(BatchItem), _I, C.POINTER(FrameInfo), _VP]),
+    "b200trk_dimp_batch_filter": (_VP, [_VP, _I]),
+    "b200trk_dimp_batch_scores": (_VP, [_VP, _I]),
+    "b200trk_dimp_batch_crop": (_VP, [_VP, _I]),
+    "b200trk_dimp_batch_state": (_I, [_VP, _I, C.POINTER(C.c_float * 9)]),
 }
 
 _lib = None

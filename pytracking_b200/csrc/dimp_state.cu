@@ -15,25 +15,28 @@ static int st_alloc(b200trk_dimp_state* s, void** p, size_t bytes) {
     return 0;
 }
 
-// The buffers both optimiser kinds share (and the GN LUTs when num_bins > 0); frees `s` on failure.
+// The buffers both optimiser kinds share (and the GN LUTs when num_bins > 0); frees `s` on failure.  filter_ext: see dimp_state.cuh.
 static int state_alloc(b200trk_dimp_state* s, b200trk_net* net, int memory_size, int filter_size, const float* label_lut,
-                       const float* mask_lut, const float* spatial_lut, int num_bins) {
+                       const float* mask_lut, const float* spatial_lut, int num_bins, float* filter_ext) {
     s->net = net; s->memory_size = memory_size; s->ksz = filter_size; s->max_batch = net->max_batch;
     s->Cc = net->dims[6]; s->Hc = net->dims[7]; s->Wc = net->dims[8];
     s->Ho = s->Hc + (filter_size + 1) % 2; s->Wo = s->Wc + (filter_size + 1) % 2;
     s->num_bins = num_bins;
     const size_t plane = (size_t)s->Cc * s->Hc * s->Wc;
     int e = 0;
-    if (!e) e = st_alloc(s, (void**)&s->filter, (size_t)s->Cc * 16 * sizeof(float));
+    if (filter_ext) s->filter = filter_ext;
+    else if (!e) e = st_alloc(s, (void**)&s->filter, (size_t)s->Cc * 16 * sizeof(float));
     s->mem_pitch = (s->Hc * s->Wc + 31) / 32 * 32;
     if (!e) e = st_alloc(s, (void**)&s->memory, (size_t)s->Cc * s->mem_pitch * memory_size * sizeof(float));
     if (!e) e = st_alloc(s, (void**)&s->boxes, (size_t)memory_size * 4 * sizeof(float));
     if (!e) e = st_alloc(s, (void**)&s->sw, (size_t)memory_size * sizeof(float));
-    if (!e) e = st_alloc(s, (void**)&s->clf, plane * s->max_batch * sizeof(float));
-    if (!e) e = st_alloc(s, (void**)&s->scores, (size_t)s->max_batch * s->Ho * s->Wo * sizeof(float));
-    if (!e) e = st_alloc(s, (void**)&s->crop, (size_t)s->max_batch * 3 * net->crop_h * net->crop_w * sizeof(float));
-    if (!e) e = st_alloc(s, (void**)&s->maxval, (size_t)s->max_batch * sizeof(float));
-    if (!e) e = st_alloc(s, (void**)&s->maxidx, (size_t)s->max_batch * 2 * sizeof(int64_t));
+    if (!filter_ext) {
+        if (!e) e = st_alloc(s, (void**)&s->clf, plane * s->max_batch * sizeof(float));
+        if (!e) e = st_alloc(s, (void**)&s->scores, (size_t)s->max_batch * s->Ho * s->Wo * sizeof(float));
+        if (!e) e = st_alloc(s, (void**)&s->crop, (size_t)s->max_batch * 3 * net->crop_h * net->crop_w * sizeof(float));
+        if (!e) e = st_alloc(s, (void**)&s->maxval, (size_t)s->max_batch * sizeof(float));
+        if (!e) e = st_alloc(s, (void**)&s->maxidx, (size_t)s->max_batch * 2 * sizeof(int64_t));
+    }
     if (!e && num_bins > 0) e = st_alloc(s, (void**)&s->luts, (size_t)3 * num_bins * sizeof(float));
     if (!e && num_bins > 0) {
         cudaError_t ce = cudaMemcpy(s->luts, label_lut, num_bins * sizeof(float), cudaMemcpyHostToDevice);
@@ -51,10 +54,9 @@ static int state_alloc(b200trk_dimp_state* s, b200trk_net* net, int memory_size,
     return e;
 }
 
-extern "C" int b200trk_dimp_state_create(b200trk_dimp_state_t** out, b200trk_net_t* net, int memory_size, int filter_size,
-                                         const float* label_lut, const float* mask_lut, const float* spatial_lut,
-                                         int num_bins, float bin_displacement, float feat_stride, float step_length,
-                                         float reg_weight, float alpha_eps) {
+int b200trk::dimp_state_create_gn(b200trk_dimp_state** out, b200trk_net* net, int memory_size, int filter_size, const float* label_lut,
+                                  const float* mask_lut, const float* spatial_lut, int num_bins, float bin_displacement, float feat_stride,
+                                  float step_length, float reg_weight, float alpha_eps, float* filter_ext) {
     B200_REQUIRE(out && net && label_lut && mask_lut && spatial_lut, "dimp_state_create: null pointer");
     B200_REQUIRE(memory_size >= 1 && memory_size <= 1024, "dimp_state_create: memory_size=%d", memory_size);
     B200_REQUIRE(filter_size == 4, "dimp_state_create: filter_size=%d not supported (4)", filter_size);
@@ -63,15 +65,23 @@ extern "C" int b200trk_dimp_state_create(b200trk_dimp_state_t** out, b200trk_net
     s->opt_kind = b200trk_dimp_state::OPT_GN;
     s->bin_displacement = bin_displacement; s->feat_stride = feat_stride;
     s->step_length = step_length; s->reg_weight = reg_weight; s->alpha_eps = alpha_eps;
-    if (int e = state_alloc(s, net, memory_size, filter_size, label_lut, mask_lut, spatial_lut, num_bins)) return e;
+    if (int e = state_alloc(s, net, memory_size, filter_size, label_lut, mask_lut, spatial_lut, num_bins, filter_ext)) return e;
     *out = s;
     return 0;
 }
 
-extern "C" int b200trk_prdimp_state_create(b200trk_dimp_state_t** out, b200trk_net_t* net, int memory_size, int filter_size,
-                                           float gauss_sigma, float feat_stride, float step_length, float reg_weight, float alpha_eps,
-                                           int has_softmax_reg, float softmax_reg, float label_threshold, int normalize_label,
-                                           float label_shrink, float uni_weight) {
+extern "C" int b200trk_dimp_state_create(b200trk_dimp_state_t** out, b200trk_net_t* net, int memory_size, int filter_size,
+                                         const float* label_lut, const float* mask_lut, const float* spatial_lut,
+                                         int num_bins, float bin_displacement, float feat_stride, float step_length,
+                                         float reg_weight, float alpha_eps) {
+    return dimp_state_create_gn(out, net, memory_size, filter_size, label_lut, mask_lut, spatial_lut, num_bins, bin_displacement,
+                                feat_stride, step_length, reg_weight, alpha_eps, nullptr);
+}
+
+int b200trk::dimp_state_create_newton(b200trk_dimp_state** out, b200trk_net* net, int memory_size, int filter_size, float gauss_sigma,
+                                      float feat_stride, float step_length, float reg_weight, float alpha_eps, int has_softmax_reg,
+                                      float softmax_reg, float label_threshold, int normalize_label, float label_shrink, float uni_weight,
+                                      float* filter_ext) {
     B200_REQUIRE(out && net, "prdimp_state_create: null pointer");
     B200_REQUIRE(memory_size >= 1 && memory_size <= 1024, "prdimp_state_create: memory_size=%d", memory_size);
     B200_REQUIRE(filter_size == 4, "prdimp_state_create: filter_size=%d not supported (4)", filter_size);
@@ -83,9 +93,17 @@ extern "C" int b200trk_prdimp_state_create(b200trk_dimp_state_t** out, b200trk_n
     s->gauss_sigma = gauss_sigma; s->has_softmax_reg = has_softmax_reg ? 1 : 0; s->softmax_reg = softmax_reg;
     s->label_threshold = label_threshold; s->normalize_label = normalize_label ? 1 : 0; s->label_shrink = label_shrink;
     s->uni_weight = uni_weight;
-    if (int e = state_alloc(s, net, memory_size, filter_size, nullptr, nullptr, nullptr, 0)) return e;
+    if (int e = state_alloc(s, net, memory_size, filter_size, nullptr, nullptr, nullptr, 0, filter_ext)) return e;
     *out = s;
     return 0;
+}
+
+extern "C" int b200trk_prdimp_state_create(b200trk_dimp_state_t** out, b200trk_net_t* net, int memory_size, int filter_size,
+                                           float gauss_sigma, float feat_stride, float step_length, float reg_weight, float alpha_eps,
+                                           int has_softmax_reg, float softmax_reg, float label_threshold, int normalize_label,
+                                           float label_shrink, float uni_weight) {
+    return dimp_state_create_newton(out, net, memory_size, filter_size, gauss_sigma, feat_stride, step_length, reg_weight, alpha_eps,
+                                    has_softmax_reg, softmax_reg, label_threshold, normalize_label, label_shrink, uni_weight, nullptr);
 }
 
 extern "C" int b200trk_dimp_state_optimizer_kind(b200trk_dimp_state_t* s) { return s ? s->opt_kind : -1; }
@@ -129,10 +147,17 @@ extern "C" int b200trk_dimp_localize_host(b200trk_dimp_state_t* s, const float* 
 int b200trk::dimp_state_update(b200trk_dimp_state* s, int scale_ind, int replace_ind, const float* target_box_host,
                                const float* sample_weights_host, int n_stored, int num_iter, cudaStream_t st) {
     B200_REQUIRE(s && target_box_host && sample_weights_host, "dimp_update: null pointer");
+    B200_REQUIRE(s->clf, "dimp_update: the state is a slot of a batch; its features are in the batch's buffer");
     B200_REQUIRE(scale_ind >= 0 && scale_ind < s->max_batch, "dimp_update: scale_ind=%d", scale_ind);
+    return dimp_state_insert(s, s->clf + (size_t)s->Cc * s->Hc * s->Wc * scale_ind, replace_ind, target_box_host, sample_weights_host,
+                             n_stored, num_iter, st);
+}
+
+int b200trk::dimp_state_insert(b200trk_dimp_state* s, const float* feat, int replace_ind, const float* target_box_host,
+                               const float* sample_weights_host, int n_stored, int num_iter, cudaStream_t st) {
+    B200_REQUIRE(s && feat && target_box_host && sample_weights_host, "dimp_update: null pointer");
     B200_REQUIRE(replace_ind >= 0 && replace_ind < s->memory_size, "dimp_update: replace_ind=%d outside memory of %d", replace_ind, s->memory_size);
     B200_REQUIRE(n_stored >= 1 && n_stored <= s->memory_size, "dimp_update: n_stored=%d", n_stored);
-    const size_t plane = (size_t)s->Cc * s->Hc * s->Wc;
     const size_t row = (size_t)s->Hc * s->Wc * sizeof(float);
     // the caller may rewrite its buffers as soon as this returns: stage the 4 + n floats in a pinned slot of our own
     const int slot = s->stage_next;
@@ -142,7 +167,7 @@ int b200trk::dimp_state_update(b200trk_dimp_state* s, int scale_ind, int replace
     for (int i = 0; i < 4; ++i) h[i] = target_box_host[i];
     for (int i = 0; i < n_stored; ++i) h[4 + i] = sample_weights_host[i];
     B200_CHECK_CUDA(cudaMemcpy2DAsync(s->memory + (size_t)s->Cc * s->mem_pitch * replace_ind, (size_t)s->mem_pitch * sizeof(float),
-                                      s->clf + plane * scale_ind, row, row, (size_t)s->Cc, cudaMemcpyDeviceToDevice, st));
+                                      feat, row, row, (size_t)s->Cc, cudaMemcpyDeviceToDevice, st));
     B200_CHECK_CUDA(cudaMemcpyAsync(s->boxes + 4 * replace_ind, h, 4 * sizeof(float), cudaMemcpyHostToDevice, st));
     B200_CHECK_CUDA(cudaMemcpyAsync(s->sw, h + 4, (size_t)n_stored * sizeof(float), cudaMemcpyHostToDevice, st));
     B200_CHECK_CUDA(cudaEventRecord(s->stage_ev[slot], st));

@@ -29,6 +29,19 @@ struct b200trk_dimp_state {
 };
 
 namespace b200trk {
+// The two state constructors behind b200trk_dimp_state_create / b200trk_prdimp_state_create.  filter_ext = NULL: the state owns its
+// filter and the crop / feature / score buffers of net->max_batch samples.  Otherwise it is one sequence of a batch (dimp_tracker.cu):
+// the filter lives at filter_ext inside the batch's [S,C,k,k] buffer and the batch owns the per-frame buffers (clf, crop, scores stay NULL).
+int dimp_state_create_gn(b200trk_dimp_state** out, b200trk_net* net, int memory_size, int filter_size, const float* label_lut,
+                         const float* mask_lut, const float* spatial_lut, int num_bins, float bin_displacement, float feat_stride,
+                         float step_length, float reg_weight, float alpha_eps, float* filter_ext);
+int dimp_state_create_newton(b200trk_dimp_state** out, b200trk_net* net, int memory_size, int filter_size, float gauss_sigma,
+                             float feat_stride, float step_length, float reg_weight, float alpha_eps, int has_softmax_reg,
+                             float softmax_reg, float label_threshold, int normalize_label, float label_shrink, float uni_weight,
+                             float* filter_ext);
+// dimp_state_update with the new sample's features given by pointer (device [C,H,W]) instead of a batch index into s->clf
+int dimp_state_insert(b200trk_dimp_state* s, const float* feat, int replace_ind, const float* target_box_host,
+                      const float* sample_weights_host, int n_stored, int num_iter, cudaStream_t st);
 int dimp_state_update(b200trk_dimp_state* s, int scale_ind, int replace_ind, const float* target_box_host,
                       const float* sample_weights_host, int n_stored, int num_iter, cudaStream_t st);
 // num_iter iterations of the state's online optimiser over the first n_stored samples of its pitched memory, filter in place

@@ -585,6 +585,15 @@ extern "C" int b200trk_dimp_tracker_initialize_host(b200trk_dimp_tracker_t* t, c
     return 0;
 }
 
+// target_neigh_sz (dimp.py:265) and prev_target_vec (dimp.py:283) of the single scale, from the state before the frame's commit
+static void loc_inputs(const b200trk_dimp_tracker* t, const b200trk_crop_geom_t& g, float neigh[2], float pv[2]) {
+    for (int i = 0; i < 2; ++i) {
+        const float output_sz = t->score_sz[i] - std::fmod(t->kernel_size[i] + 1.0f, 2.0f);
+        neigh[i] = (f32(t->p.target_neighborhood_scale) * (t->target_sz[i] / g.sample_scale)) * (output_sz / t->img_sample_sz[i]);
+        pv[i] = (t->pos[i] - g.sample_pos[i]) / ((t->img_sample_sz[i] / output_sz) * g.sample_scale);
+    }
+}
+
 static int track_frame(b200trk_dimp_tracker* t, const uint8_t* image, bool on_device, int H, int W, b200trk_frame_info_t* info,
                        b200trk_stream_t stream) {
     B200_REQUIRE(t && image && info, "dimp_track_host: null pointer");
@@ -601,13 +610,8 @@ static int track_frame(b200trk_dimp_tracker* t, const uint8_t* image, bool on_de
     if (int e = b200trk_sample_patch(on_device ? image : t->img_dev, H, W, &g, iss, iss, s->crop, stream)) return e;
     if (int e = b200trk_net_forward(s->net, s->crop, 1, nullptr, nullptr, s->clf, stream)) return e;
     if (int e = b200trk_apply_filter(s->clf, s->filter, s->scores, 1, s->Cc, s->Hc, s->Wc, s->ksz, nullptr, nullptr, stream)) return e;
-    // target_neigh_sz (dimp.py:265) and prev_target_vec (dimp.py:283) of the single scale
     float neigh[2], pv[2];
-    for (int i = 0; i < 2; ++i) {
-        const float output_sz = t->score_sz[i] - std::fmod(t->kernel_size[i] + 1.0f, 2.0f);
-        neigh[i] = (f32(t->p.target_neighborhood_scale) * (t->target_sz[i] / g.sample_scale)) * (output_sz / t->img_sample_sz[i]);
-        pv[i] = (t->pos[i] - g.sample_pos[i]) / ((t->img_sample_sz[i] / output_sz) * g.sample_scale);
-    }
+    loc_inputs(t, g, neigh, pv);
     if (int e = b200trk_dimp_localize(s->scores, 1, s->Ho, s->Wo, &t->p, neigh, pv, t->loc_dev, stream)) return e;
     B200_CHECK_CUDA(cudaMemcpyAsync(t->loc_host, t->loc_dev, sizeof(b200trk_loc_result_t), cudaMemcpyDeviceToHost, st));
     B200_CHECK_CUDA(cudaStreamSynchronize(st));
@@ -644,4 +648,265 @@ extern "C" int b200trk_dimp_track_host(b200trk_dimp_tracker_t* t, const uint8_t*
 extern "C" int b200trk_dimp_track_device(b200trk_dimp_tracker_t* t, const uint8_t* image_dev, int H, int W, b200trk_frame_info_t* info,
                                          b200trk_stream_t stream) {
     return track_frame(t, image_dev, true, H, W, info, stream);
+}
+
+// ---------------------------------------------------------------------------------------------------------------------------
+// batch of sequences: S per-sequence trackers on one network, one crop / forward / classify / localisation launch per step
+// ---------------------------------------------------------------------------------------------------------------------------
+// The forward always runs at batch S, idle and released slots included: the convolution plans (tile shape, split-K) depend on the batch
+// size and every output tile belongs to one sample, so a sequence's bits depend on its own frames and on S only -- never on its
+// batch-mates, its slot or when they started -- and the network's cached graph (keyed on pointers and S) is replayed every step.
+// The online optimiser stays per sequence (dimp_state_insert / dimp_state_optimize on the slot's state), enqueued back to back.
+struct b200trk_dimp_batch {
+    b200trk_net* net = nullptr;
+    int cap = 0, Cc = 0, Hc = 0, Wc = 0, Ho = 0, Wo = 0, ksz = 4, iss = 0;
+    b200trk_dimp_params_t p;
+    b200trk_dimp_tracker* t[kBatchMax] = {};
+    b200trk_dimp_state* st[kBatchMax] = {};
+    float *crop = nullptr, *clf = nullptr, *scores = nullptr, *filters = nullptr;   // device [S,3,iss,iss] [S,C,Hc,Wc] [S,Ho,Wo] [S,C,k,k]
+    uint8_t* img_dev = nullptr; size_t img_cap = 0;                                  // the step's uploaded frames, back to back
+    cudaStream_t copy_stream = nullptr; cudaEvent_t ev_img = nullptr;
+    b200trk_loc_result_t* loc_dev = nullptr;                                         // [S]
+    b200trk_loc_result_t* loc_host = nullptr;                                        // pinned [S]
+};
+
+extern "C" int b200trk_dimp_batch_destroy(b200trk_dimp_batch_t* b) {
+    if (!b) return 0;
+    for (int i = 0; i < kBatchMax; ++i) {
+        if (b->t[i]) b200trk_dimp_tracker_destroy(b->t[i]);
+        if (b->st[i]) b200trk_dimp_state_destroy(b->st[i]);
+    }
+    for (void* q : {(void*)b->crop, (void*)b->clf, (void*)b->scores, (void*)b->filters, (void*)b->img_dev, (void*)b->loc_dev}) if (q) cudaFree(q);
+    if (b->loc_host) cudaFreeHost(b->loc_host);
+    if (b->copy_stream) cudaStreamDestroy(b->copy_stream);
+    if (b->ev_img) cudaEventDestroy(b->ev_img);
+    delete b;
+    return 0;
+}
+
+template <class MakeState>
+static int batch_create(b200trk_dimp_batch** out, b200trk_net* net, int capacity, const b200trk_dimp_params_t* params, int filter_size,
+                        MakeState make_state) {
+    B200_REQUIRE(out && net && params, "dimp_batch_create: null pointer");
+    B200_REQUIRE(capacity >= 1 && capacity <= kBatchMax, "dimp_batch_create: capacity=%d outside 1..%d", capacity, kBatchMax);
+    B200_REQUIRE(!params->use_iou_net, "dimp_batch_create: use_iou_net is not supported in a batch (the native IoUNet needs each "
+                 "sequence's modulation vectors from the reference's initialisation); set use_iou_net = False");
+    B200_REQUIRE(params->border_mode != 1, "dimp_batch_create: border_mode 'inside' changes the initial sample, which the native "
+                 "initialisation does not implement");
+    B200_REQUIRE(filter_size == 4, "dimp_batch_create: filter_size=%d not supported (4)", filter_size);
+    B200_REQUIRE(net->max_batch >= capacity, "dimp_batch_create: the network was built for batches of %d, capacity=%d", net->max_batch, capacity);
+    b200trk_dimp_batch* b = new b200trk_dimp_batch();
+    b->net = net; b->cap = capacity; b->p = *params; b->ksz = filter_size; b->iss = params->image_sample_size;
+    b->Cc = net->dims[6]; b->Hc = net->dims[7]; b->Wc = net->dims[8];
+    b->Ho = b->Hc + (filter_size + 1) % 2; b->Wo = b->Wc + (filter_size + 1) % 2;
+    const size_t S = (size_t)capacity, fsz = (size_t)b->Cc * filter_size * filter_size;
+    auto fail = [&](int e) { b200trk_dimp_batch_destroy(b); return e ? e : 1; };
+    auto alloc = [&](void** q, size_t bytes) {
+        return cudaMalloc(q, bytes) == cudaSuccess && cudaMemset(*q, 0, bytes) == cudaSuccess;
+    };
+    if (!alloc((void**)&b->crop, S * 3 * net->crop_h * net->crop_w * sizeof(float)) ||
+        !alloc((void**)&b->clf, S * b->Cc * b->Hc * b->Wc * sizeof(float)) || !alloc((void**)&b->scores, S * b->Ho * b->Wo * sizeof(float)) ||
+        !alloc((void**)&b->filters, S * fsz * sizeof(float)) || !alloc((void**)&b->loc_dev, S * sizeof(b200trk_loc_result_t)) ||
+        cudaMallocHost((void**)&b->loc_host, S * sizeof(b200trk_loc_result_t)) != cudaSuccess ||
+        cudaStreamCreateWithFlags(&b->copy_stream, cudaStreamNonBlocking) != cudaSuccess ||
+        cudaEventCreateWithFlags(&b->ev_img, cudaEventDisableTiming) != cudaSuccess) {
+        set_error("dimp_batch_create: allocation failed");
+        return fail(1);
+    }
+    for (int i = 0; i < capacity; ++i) {
+        if (int e = make_state(b->filters + i * fsz, &b->st[i])) return fail(e);
+        if (int e = b200trk_dimp_tracker_create(&b->t[i], b->st[i], params)) return fail(e);
+    }
+    *out = b;
+    return 0;
+}
+
+extern "C" int b200trk_dimp_batch_create(b200trk_dimp_batch_t** out, b200trk_net_t* net, int capacity, const b200trk_dimp_params_t* params,
+                                         int filter_size, const float* label_lut, const float* mask_lut, const float* spatial_lut, int num_bins,
+                                         float bin_displacement, float feat_stride, float step_length, float reg_weight, float alpha_eps) {
+    B200_REQUIRE(params, "dimp_batch_create: null pointer");
+    return batch_create(out, net, capacity, params, filter_size, [&](float* filter, b200trk_dimp_state** s) {
+        return dimp_state_create_gn(s, net, params->sample_memory_size, filter_size, label_lut, mask_lut, spatial_lut, num_bins,
+                                    bin_displacement, feat_stride, step_length, reg_weight, alpha_eps, filter);
+    });
+}
+
+extern "C" int b200trk_prdimp_batch_create(b200trk_dimp_batch_t** out, b200trk_net_t* net, int capacity, const b200trk_dimp_params_t* params,
+                                           int filter_size, float gauss_sigma, float feat_stride, float step_length, float reg_weight,
+                                           float alpha_eps, int has_softmax_reg, float softmax_reg, float label_threshold, int normalize_label,
+                                           float label_shrink, float uni_weight) {
+    B200_REQUIRE(params, "prdimp_batch_create: null pointer");
+    return batch_create(out, net, capacity, params, filter_size, [&](float* filter, b200trk_dimp_state** s) {
+        return dimp_state_create_newton(s, net, params->sample_memory_size, filter_size, gauss_sigma, feat_stride, step_length, reg_weight,
+                                        alpha_eps, has_softmax_reg, softmax_reg, label_threshold, normalize_label, label_shrink, uni_weight,
+                                        filter);
+    });
+}
+
+static int batch_slot_ok(const b200trk_dimp_batch* b, int slot, const char* what) {
+    B200_REQUIRE(b, "%s: null pointer", what);
+    B200_REQUIRE(slot >= 0 && slot < b->cap, "%s: slot %d outside 0..%d", what, slot, b->cap - 1);
+    return 0;
+}
+
+extern "C" int b200trk_dimp_batch_release(b200trk_dimp_batch_t* b, int slot) {
+    if (int e = batch_slot_ok(b, slot, "dimp_batch_release")) return e;
+    b->t[slot]->initialized = 0;       // the slot's device state is overwritten by the next sequence's initialisation
+    return 0;
+}
+
+extern "C" float* b200trk_dimp_batch_filter(b200trk_dimp_batch_t* b, int slot) {
+    return batch_slot_ok(b, slot, "dimp_batch_filter") ? nullptr : b->filters + (size_t)slot * b->Cc * b->ksz * b->ksz;
+}
+extern "C" float* b200trk_dimp_batch_scores(b200trk_dimp_batch_t* b, int slot) {
+    return batch_slot_ok(b, slot, "dimp_batch_scores") ? nullptr : b->scores + (size_t)slot * b->Ho * b->Wo;
+}
+extern "C" float* b200trk_dimp_batch_crop(b200trk_dimp_batch_t* b, int slot) {
+    return batch_slot_ok(b, slot, "dimp_batch_crop") ? nullptr : b->crop + (size_t)slot * 3 * b->iss * b->iss;
+}
+extern "C" int b200trk_dimp_batch_state(const b200trk_dimp_batch_t* b, int slot, float out[9]) {
+    if (int e = batch_slot_ok(b, slot, "dimp_batch_state")) return e;
+    return b200trk_dimp_tracker_state(b->t[slot], out);
+}
+
+static int batch_step(b200trk_dimp_batch* b, const b200trk_batch_item_t* items, int n, bool on_device, b200trk_frame_info_t* infos,
+                      b200trk_stream_t stream) {
+    B200_REQUIRE(b && items && infos, "dimp_batch_step: null pointer");
+    B200_REQUIRE(n >= 1 && n <= b->cap, "dimp_batch_step: %d items for a batch of %d slots", n, b->cap);
+    // every refusal before any state changes
+    bool seen[kBatchMax] = {};
+    for (int k = 0; k < n; ++k) {
+        const b200trk_batch_item_t& it = items[k];
+        B200_REQUIRE(it.slot >= 0 && it.slot < b->cap, "dimp_batch_step: slot %d outside 0..%d", it.slot, b->cap - 1);
+        B200_REQUIRE(!seen[it.slot], "dimp_batch_step: slot %d appears twice in one step", it.slot);
+        seen[it.slot] = true;
+        B200_REQUIRE(it.image && it.H > 0 && it.W > 0, "dimp_batch_step: slot %d: no frame or an empty one (%dx%d)", it.slot, it.H, it.W);
+        const b200trk_dimp_tracker* t = b->t[it.slot];
+        if (it.init) {
+            B200_REQUIRE(it.init_bbox[2] > 0 && it.init_bbox[3] > 0, "dimp_batch_step: slot %d: init box of size %gx%g", it.slot,
+                         it.init_bbox[2], it.init_bbox[3]);
+        } else {
+            B200_REQUIRE(t->initialized, "dimp_batch_step: slot %d is not tracking a sequence (never initialised, or released)", it.slot);
+            B200_REQUIRE((float)it.H == t->image_sz[0] && (float)it.W == t->image_sz[1],
+                         "dimp_batch_step: slot %d: frame is %dx%d, its sequence started with %dx%d", it.slot, it.H, it.W,
+                         (int)t->image_sz[0], (int)t->image_sz[1]);
+        }
+    }
+    cudaStream_t st = (cudaStream_t)stream;
+    const int iss = b->iss;
+    // 1. crop plans on the host
+    b200trk_crop_geom_t g[kBatchMax];
+    float box[kBatchMax][4];
+    for (int k = 0; k < n; ++k) {
+        const b200trk_batch_item_t& it = items[k];
+        if (it.init) { if (int e = b200trk_dimp_tracker_init_state(b->t[it.slot], it.H, it.W, it.init_bbox, &g[k], box[k])) return e; }
+        else if (int e = b200trk_dimp_tracker_plan_crop(b->t[it.slot], &g[k])) return e;
+        B200_REQUIRE(g[k].win_r >= 0 && g[k].win_c >= 0 && g[k].win_r + iss <= g[k].out_h && g[k].win_c + iss <= g[k].out_w && g[k].df >= 1 &&
+                     g[k].in_h >= 1 && g[k].in_w >= 1, "dimp_batch_step: slot %d: bad crop geometry", it.slot);
+    }
+    // 2. the frames, on the copy stream behind one event (the previous step's crop kernel finished before it returned)
+    SampleBatchArgs sa;
+    size_t off[kBatchMax], total = 0;
+    for (int k = 0; k < n; ++k) { off[k] = total; total += ((size_t)items[k].H * items[k].W * 3 + 255) / 256 * 256; }
+    if (!on_device) {
+        if (total > b->img_cap) {
+            if (b->img_dev) B200_CHECK_CUDA(cudaFree(b->img_dev));
+            b->img_dev = nullptr; b->img_cap = 0;
+            B200_CHECK_CUDA(cudaMalloc((void**)&b->img_dev, total));
+            b->img_cap = total;
+        }
+        for (int k = 0; k < n; ++k)
+            B200_CHECK_CUDA(cudaMemcpyAsync(b->img_dev + off[k], items[k].image, (size_t)items[k].H * items[k].W * 3, cudaMemcpyHostToDevice,
+                                            b->copy_stream));
+        B200_CHECK_CUDA(cudaEventRecord(b->ev_img, b->copy_stream));
+        B200_CHECK_CUDA(cudaStreamWaitEvent(st, b->ev_img, 0));
+    }
+    for (int k = 0; k < n; ++k) {
+        sa.im[k] = on_device ? items[k].image : b->img_dev + off[k];
+        sa.H[k] = items[k].H; sa.W[k] = items[k].W; sa.dst[k] = items[k].slot; sa.g[k] = g[k];
+    }
+    // 3. one crop launch for every item
+    sample_patch_batch_kernel<<<dim3((iss + 31) / 32, (iss + 7) / 8, n), 256, 0, st>>>(sa, iss, b->crop);
+    B200_LAUNCH_CHECK();
+    // 4. one forward at batch S
+    if (int e = b200trk_net_forward(b->net, b->crop, b->cap, nullptr, nullptr, b->clf, stream)) return e;
+    // 5. one classify launch, every slot with its own filter
+    {
+        constexpr int SL18 = CorrSlots<18>::value, SL22 = CorrSlots<22>::value;
+        B200_REQUIRE(b->Hc == b->Wc && (b->Hc == 18 || b->Hc == 22), "dimp_batch_step: feature size %dx%d not supported (18x18, 22x22)", b->Hc, b->Wc);
+        const int slots = b->Hc == 18 ? SL18 : SL22;
+        B200_REQUIRE(b->Cc % slots == 0, "dimp_batch_step: C=%d must be a multiple of %d", b->Cc, slots);
+        const int NCH = b->Cc / slots;
+        const int npos = b->Ho * b->Wo;
+        char* ws = (char*)workspace(4096 + (size_t)b->cap * NCH * npos * sizeof(float), 0);     // as apply_filter: counters, then partial maps
+        if (!ws) return 3;
+        const size_t fstride = (size_t)b->Cc * b->ksz * b->ksz;
+        auto launch = [&](auto kern, int nthreads, size_t smem) -> int {
+            B200_CHECK_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+            kern<<<dim3(NCH, b->cap), nthreads, smem, st>>>(b->clf, b->filters, fstride, b->scores, (float*)(ws + 4096), (unsigned*)ws, b->Cc);
+            B200_LAUNCH_CHECK();
+            return 0;
+        };
+        if (int e = b->Hc == 18 ? launch(classify_batch_kernel<18, SL18>, CorrCta<18, SL18>::NTHREADS, classify_smem_bytes<18, SL18>())
+                                : launch(classify_batch_kernel<22, SL22>, CorrCta<22, SL22>::NTHREADS, classify_smem_bytes<22, SL22>())) return e;
+    }
+    // 6. one localisation launch, one CTA per tracked item; 7. one D2H and one synchronisation
+    LocBatchArgs la;
+    la.a = make_loc_args(1, b->Ho, b->Wo, &b->p, nullptr, nullptr);
+    int tracked[kBatchMax], nt = 0;
+    for (int k = 0; k < n; ++k) {
+        if (items[k].init) continue;
+        la.slot[nt] = items[k].slot;
+        loc_inputs(b->t[items[k].slot], g[k], la.neigh[nt], la.prev_vec[nt]);
+        tracked[nt++] = k;
+    }
+    if (nt > 0) {
+        const size_t smem = loc_smem_bytes(la.a);
+        B200_REQUIRE(smem <= 48 * 1024, "dimp_batch_step: score pre-processing holds Ho*Wo=%d floats in shared memory", b->Ho * b->Wo);
+        localize_batch_kernel<<<nt, 256, smem, st>>>(b->scores, la, b->loc_dev);
+        B200_LAUNCH_CHECK();
+        B200_CHECK_CUDA(cudaMemcpyAsync(b->loc_host, b->loc_dev, (size_t)nt * sizeof(b200trk_loc_result_t), cudaMemcpyDeviceToHost, st));
+    }
+    B200_CHECK_CUDA(cudaStreamSynchronize(st));
+    // 8. the host half of every tracked frame; 9. each slot's memory insert and optimiser call, back to back on the stream
+    const size_t plane = (size_t)b->Cc * b->Hc * b->Wc;
+    for (int j = 0; j < nt; ++j) {
+        const int k = tracked[j], slot = items[k].slot;
+        b200trk_dimp_tracker* t = b->t[slot];
+        b200trk_frame_info_t* info = &infos[k];
+        if (int e = b200trk_dimp_tracker_commit_localize(t, &g[k], &b->loc_host[j], info)) return e;
+        if (int e = b200trk_dimp_tracker_commit_update(t, &g[k], info, nullptr)) return e;
+        if (info->updated) {
+            if (int e = dimp_state_insert(b->st[slot], b->clf + plane * slot, info->replace_ind, info->target_box, t->sw.data(), info->n_stored,
+                                          info->num_iter, st)) return e;
+        } else if (info->num_iter > 0) {
+            if (int e = dimp_state_optimize(b->st[slot], info->n_stored, info->num_iter, st)) return e;
+        }
+    }
+    // initialisation (b200trk_dimp_tracker_initialize_host): net_opt_iter iterations from the zero filter on the one init sample
+    for (int k = 0; k < n; ++k) {
+        if (!items[k].init) continue;
+        const int slot = items[k].slot;
+        b200trk_dimp_state* s = b->st[slot];
+        b200trk_frame_info_t* info = &infos[k];
+        std::memset(info, 0, sizeof(*info));
+        info->crop = g[k];
+        for (int i = 0; i < 4; ++i) { info->bbox[i] = f32(items[k].init_bbox[i]); info->target_box[i] = box[k][i]; }
+        info->updated = 1; info->n_stored = 1; info->num_iter = b->p.net_opt_iter > 0 ? b->p.net_opt_iter : 0;
+        B200_CHECK_CUDA(cudaMemsetAsync(s->filter, 0, (size_t)s->Cc * s->ksz * s->ksz * sizeof(float), st));
+        B200_CHECK_CUDA(cudaMemsetAsync(s->sw, 0, (size_t)s->memory_size * sizeof(float), st));
+        const float one = 1.f;
+        if (int e = dimp_state_insert(s, b->clf + plane * slot, 0, box[k], &one, 1, info->num_iter, st)) return e;
+    }
+    return 0;
+}
+
+extern "C" int b200trk_dimp_batch_step_host(b200trk_dimp_batch_t* b, const b200trk_batch_item_t* items, int n, b200trk_frame_info_t* infos,
+                                            b200trk_stream_t stream) {
+    return batch_step(b, items, n, false, infos, stream);
+}
+
+extern "C" int b200trk_dimp_batch_step_device(b200trk_dimp_batch_t* b, const b200trk_batch_item_t* items, int n, b200trk_frame_info_t* infos,
+                                              b200trk_stream_t stream) {
+    return batch_step(b, items, n, true, infos, stream);
 }

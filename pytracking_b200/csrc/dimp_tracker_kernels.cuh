@@ -3,7 +3,10 @@
 // arithmetic, kept in a header of their own so that the SAME source also compiles as host code under tests/cpu_emul/cuda_shim.h:
 // tests/test_dimp_kernels_cpu.py runs the sampler against torch-CPU bilinear interpolation (bit-exact) and the localisation kernel
 // against the decisions recorded from the unmodified reference tracker, on the CPU.  Included by dimp_tracker.cu only.
+// The batch of sequences (b200trk_dimp_batch_*) runs the same per-pixel / per-map bodies in one launch per stage: sample_patch_batch_kernel,
+// classify_batch_kernel and localize_batch_kernel (tests/test_batch_kernels_cpu.py runs them against the single-sequence kernels).
 #pragma once
+#include "corr.cuh"
 
 // ---------------------------------------------------------------------------------------------------------------------------
 // sample_patch on the device
@@ -26,11 +29,9 @@ __device__ __forceinline__ void linear_src(int o, int in_size, int out_size, flo
     w1 = l1;
 }
 
-__global__ void __launch_bounds__(256) sample_patch_kernel(const uint8_t* __restrict__ im, int H, int W, b200trk_crop_geom_t g,
-                                                           int win_h, int win_w, float* __restrict__ out) {
-    const int ox = blockIdx.x * 32 + (threadIdx.x & 31);
-    const int oy = blockIdx.y * 8 + (threadIdx.x >> 5);
-    if (ox >= win_w || oy >= win_h) return;
+// One output pixel (ox, oy) of the [3, win_h, win_w] window, all three channels
+__device__ __forceinline__ void sample_patch_px(const uint8_t* __restrict__ im, int H, int W, const b200trk_crop_geom_t& g, int win_h, int win_w,
+                                                float* __restrict__ out, int ox, int oy) {
     const int H2 = (H - g.os_r + g.df - 1) / g.df, W2 = (W - g.os_c + g.df - 1) / g.df;      // im[..., os::df, os::df]
     const float sh = __fdiv_rn((float)g.in_h, (float)g.out_h), sw = __fdiv_rn((float)g.in_w, (float)g.out_w);
     int y0, y1, x0, x1; float wy0, wy1, wx0, wx1;
@@ -55,6 +56,31 @@ __global__ void __launch_bounds__(256) sample_patch_kernel(const uint8_t* __rest
         }
         out[((size_t)ch * win_h + oy) * win_w + ox] = v;
     }
+}
+
+__global__ void __launch_bounds__(256) sample_patch_kernel(const uint8_t* __restrict__ im, int H, int W, b200trk_crop_geom_t g,
+                                                           int win_h, int win_w, float* __restrict__ out) {
+    const int ox = blockIdx.x * 32 + (threadIdx.x & 31);
+    const int oy = blockIdx.y * 8 + (threadIdx.x >> 5);
+    if (ox >= win_w || oy >= win_h) return;
+    sample_patch_px(im, H, W, g, win_h, win_w, out, ox, oy);
+}
+
+// The crops of a batch of sequences in one launch: item blockIdx.z samples its own frame with its own geometry (the windowed
+// first-frame crop included) into crop `dst` of the [S, 3, win, win] buffer, pixel for pixel as sample_patch_kernel does.
+constexpr int kBatchMax = 16;
+struct SampleBatchArgs {
+    const uint8_t* im[kBatchMax];
+    int H[kBatchMax], W[kBatchMax], dst[kBatchMax];
+    b200trk_crop_geom_t g[kBatchMax];
+};
+
+__global__ void __launch_bounds__(256) sample_patch_batch_kernel(SampleBatchArgs a, int win, float* __restrict__ out) {
+    const int b = blockIdx.z;
+    const int ox = blockIdx.x * 32 + (threadIdx.x & 31);
+    const int oy = blockIdx.y * 8 + (threadIdx.x >> 5);
+    if (ox >= win || oy >= win) return;
+    sample_patch_px(a.im[b], a.H[b], a.W[b], a.g[b], win, win, out + (size_t)a.dst[b] * 3 * win * win, ox, oy);
 }
 
 // ---------------------------------------------------------------------------------------------------------------------------
@@ -127,7 +153,7 @@ __device__ __forceinline__ float loc_block_sum(float v, float* red) {
 #else
 #define B200_LOC_DYN_SMEM(name) extern __shared__ float name[]
 #endif
-__global__ void __launch_bounds__(256) localize_kernel(const float* __restrict__ scores_in, LocArgs a, b200trk_loc_result_t* __restrict__ res) {
+__device__ __forceinline__ void localize_body(const float* __restrict__ scores_in, LocArgs a, b200trk_loc_result_t* __restrict__ res) {
     __shared__ AM red[8];
     const int n = a.Ho * a.Wo;
     const AM none = {__int_as_float(0xff800000), 1 << 30, 1 << 30};
@@ -211,6 +237,73 @@ __global__ void __launch_bounds__(256) localize_kernel(const float* __restrict__
         }
     }
     if (threadIdx.x == 0) *res = out;
+}
+
+__global__ void __launch_bounds__(256) localize_kernel(const float* __restrict__ scores_in, LocArgs a, b200trk_loc_result_t* __restrict__ res) {
+    localize_body(scores_in, a, res);
+}
+
+// One localisation per tracked sequence of a batch: CTA i runs localize_kernel's body (one scale) on the score map of slot[i], with that
+// sequence's target neighbourhood and previous target vector, and writes result i.
+struct LocBatchArgs {
+    LocArgs a;                                   // the parameters the sequences share; S = 1
+    int slot[kBatchMax];
+    float neigh[kBatchMax][2], prev_vec[kBatchMax][2];
+};
+
+__global__ void __launch_bounds__(256) localize_batch_kernel(const float* __restrict__ scores, LocBatchArgs b, b200trk_loc_result_t* __restrict__ res) {
+    const int i = blockIdx.x;
+    LocArgs a = b.a;
+    for (int k = 0; k < 2; ++k) { a.neigh[0][k] = b.neigh[i][k]; a.prev_vec[0][k] = b.prev_vec[i][k]; }
+    localize_body(scores + (size_t)b.slot[i] * a.Ho * a.Wo, a, res + i);
+}
+
+// ---------------------------------------------------------------------------------------------------------------------------
+// classify for a batch of sequences: one 4x4 filter per sample
+// ---------------------------------------------------------------------------------------------------------------------------
+// apply_filter_kernel (corr_kernels.cuh) as b200trk_apply_filter runs it for ONE sample (passes = 1, no arg-max), on sample blockIdx.y of
+// [n,C,FS,FS] with the filter filt + blockIdx.y * filt_stride: the same sweep, the same partial maps and the same fixed-order sum, so every
+// sample's scores carry the bits of a single-sample apply_filter call with its own filter.  Grid (C / SLOTS, n).
+template <int FS, int SLOTS>
+__global__ void __launch_bounds__(b200trk::CorrCta<FS, SLOTS>::NTHREADS)
+classify_batch_kernel(const float* __restrict__ feat, const float* __restrict__ filt, size_t filt_stride, float* __restrict__ scores,
+                      float* part, unsigned* counters, int C) {
+    using K = b200trk::CorrCta<FS, SLOTS>;
+    using G = b200trk::CorrGeom<FS>;
+    B200_LOC_DYN_SMEM(smem);
+    float* planes = smem;
+    float* red = planes + K::PLANES_FLOATS;
+    float* vec = red + K::RED_FLOATS;                 // [SLOTS*16]
+    __shared__ int s_last;
+
+    const int NCH = gridDim.x, chunk = blockIdx.x, i = blockIdx.y;
+    K::zero_planes(planes);
+    const float* f = filt + (size_t)i * filt_stride;
+    for (int o = threadIdx.x; o < SLOTS * 16; o += K::NTHREADS) vec[o] = f[(size_t)chunk * SLOTS * 16 + o];
+    __syncthreads();
+
+    typename K::Ctx cx{feat + (size_t)i * C * G::FPLANE, C, 1, chunk * SLOTS, 1, 0, 1};   // sample i alone
+    K::sweep_apply(cx, planes, red, vec, part + ((size_t)i * NCH + chunk) * G::NPOS, (size_t)NCH * G::NPOS);
+
+    __threadfence();
+    __syncthreads();
+    if (threadIdx.x == 0) s_last = (atomicAdd(&counters[i], 1u) == (unsigned)(NCH - 1));
+    __syncthreads();
+    if (!s_last) return;
+    __threadfence();
+    for (int pos = threadIdx.x; pos < G::NPOS; pos += K::NTHREADS) {
+        float s = 0.f;
+        for (int ch = 0; ch < NCH; ++ch) s += __ldcg(part + ((size_t)i * NCH + ch) * G::NPOS + pos);
+        scores[(size_t)i * G::NPOS + pos] = s;
+    }
+    if (threadIdx.x == 0) counters[i] = 0;   // self-reset for the next call
+}
+
+// dynamic shared memory of classify_batch_kernel
+template <int FS, int SLOTS>
+inline size_t classify_smem_bytes() {
+    using K = b200trk::CorrCta<FS, SLOTS>;
+    return (size_t)(K::PLANES_FLOATS + K::RED_FLOATS + SLOTS * 16) * sizeof(float);
 }
 
 // LocArgs from the tracker parameters, as b200trk_dimp_localize passes them to localize_kernel (host)

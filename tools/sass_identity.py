@@ -16,7 +16,10 @@ def funcs(so):
     out = {}
     for p in re.split(r"\n(?=\t\tFunction : )", txt)[1:]:
         name = re.sub(r"_GLOBAL__N__[0-9a-f]{8}_", "_GLOBAL__N__HASH_", p.split("\n", 1)[0].strip().replace("Function : ", ""))
-        out[name] = re.split(r"\n(?=Fatbin|\s*\.\.\.\.|code for sm)", p.split("\n", 1)[1])[0].strip()
+        body = re.split(r"\n(?=Fatbin|\s*\.\.\.\.|code for sm)", p.split("\n", 1)[1])[0].strip()
+        # cuobjdump pads its columns to the longest instruction of the whole cubin, so a kernel added to a translation unit re-pads
+        # the listing of its unchanged neighbours: compare instructions and encodings, not the padding
+        out[name] = re.sub(r"[ \t]+", " ", body)
     return out
 
 
