@@ -13,8 +13,8 @@ import torch
 
 from . import _lib
 from .engine import BackboneEngine
-from .frame_engine import _view, newton_scalars
-from .tracker import make_params, newton_hparams
+from .frame_engine import _view, optimizer_args
+from .tracker import frame_pointer, tracker_settings
 
 
 class DiMPBatchTracker:
@@ -22,41 +22,21 @@ class DiMPBatchTracker:
     optimiser, whose softmax_reg the localisation then uses).  use_iou_net must be False."""
 
     def __init__(self, state_dict, params, capacity, arch="resnet50", newton=None, device=None, precision=0, **param_overrides):
-        self.params = params if isinstance(params, _lib.DimpParams) else make_params(params, **param_overrides)
+        self.params, newton = tracker_settings(params, newton, **param_overrides)
         p = self.params
         if p.use_iou_net:
             raise RuntimeError("DiMPBatchTracker: use_iou_net is not supported in a batch; set use_iou_net=False")
         if not 1 <= int(capacity) <= 16:
             raise RuntimeError("DiMPBatchTracker: capacity=%r outside 1..16" % (capacity,))
         self.capacity = int(capacity)
-        if newton is not None:
-            src = None if isinstance(params, _lib.DimpParams) else params
-            newton = newton_hparams(newton, src, **param_overrides)
-            p.has_softmax_reg = int(newton["softmax_reg"] is not None)
-            p.softmax_reg = 0.0 if newton["softmax_reg"] is None else float(newton["softmax_reg"])
         self.backbone = BackboneEngine(state_dict, arch, 4, self.capacity, p.image_sample_size, precision, device)
         self.device = self.backbone.device
+        args, _, _ = optimizer_args(state_dict, newton)
+        create = "dimp_batch_create" if newton is None else "prdimp_batch_create"
         h = C.c_void_p()
-        L = _lib.lib()
         with torch.cuda.device(self.device):
-            if newton is None:
-                po = "classifier.filter_optimizer."
-                luts = [state_dict[po + k].detach().float().reshape(-1).contiguous().cpu() for k in
-                        ("label_map_predictor.weight", "target_mask_predictor.0.weight", "spatial_weight_predictor.weight")]
-                step_length = float(torch.exp(state_dict[po + "log_step_length"].float()).item())
-                reg_weight = max(float(state_dict[po + "filter_reg"].float().item()) ** 2, 1e-3 ** 2)
-                _lib.check(L.b200trk_dimp_batch_create(C.byref(h), self.backbone.handle, self.capacity, C.byref(p), 4,
-                                                       C.c_void_p(luts[0].data_ptr()), C.c_void_p(luts[1].data_ptr()),
-                                                       C.c_void_p(luts[2].data_ptr()), luts[0].numel(), 0.1, 16.0, step_length,
-                                                       reg_weight, 0.0), "dimp_batch_create")
-            else:
-                step_length, reg_weight = newton_scalars(state_dict, newton)
-                sreg = newton["softmax_reg"]
-                _lib.check(L.b200trk_prdimp_batch_create(
-                    C.byref(h), self.backbone.handle, self.capacity, C.byref(p), 4, float(newton["gauss_sigma"]),
-                    float(newton["feat_stride"]), step_length, reg_weight, float(newton["alpha_eps"]), int(sreg is not None),
-                    0.0 if sreg is None else float(sreg), float(newton["label_threshold"]), int(bool(newton["normalize_label"])),
-                    float(newton["label_shrink"]), float(newton["init_uni_weight"] or 0.0)), "prdimp_batch_create")
+            _lib.check(getattr(_lib.lib(), "b200trk_" + create)(C.byref(h), self.backbone.handle, self.capacity, C.byref(p), 4, *args),
+                       create)
         self.handle = h
         cc, hc, wc = self.backbone.dims[6:9]
         self.feat_dims = (cc, hc, wc)
@@ -68,18 +48,6 @@ class DiMPBatchTracker:
 
     def _stream(self):
         return C.c_void_p(torch.cuda.current_stream(self.device).cuda_stream)
-
-    def _host_frame(self, slot, image):
-        if isinstance(image, torch.Tensor) and not image.is_cuda and image.is_pinned():
-            return image, image.data_ptr()
-        a = np.ascontiguousarray(image)
-        if a.dtype != np.uint8 or a.ndim != 3 or a.shape[2] != 3:
-            raise RuntimeError("DiMPBatchTracker: frames must be uint8 [H,W,3] (RGB), got %s %s" % (a.dtype, a.shape))
-        buf = self._pinned.get(slot)
-        if buf is None or tuple(buf.shape) != a.shape:
-            buf = self._pinned[slot] = torch.empty(a.shape, dtype=torch.uint8).pin_memory()
-        buf.numpy()[...] = a
-        return buf, buf.data_ptr()
 
     def step(self, frames):
         """frames: {slot: (frame, init_info_or_None)}.  init_info = {'init_bbox': [x, y, w, h]} starts a sequence in the slot; None
@@ -93,19 +61,12 @@ class DiMPBatchTracker:
         on_device = None
         for k, (slot, (frame, init)) in enumerate(frames.items()):
             it = self._items[k]
-            dev = isinstance(frame, torch.Tensor) and frame.is_cuda
+            buf, ptr, H, W, dev = frame_pointer(frame, self._pinned, slot, "DiMPBatchTracker.step")
+            keep.append(buf)
             if on_device is None:
                 on_device = dev
             elif on_device != dev:
                 raise RuntimeError("DiMPBatchTracker.step: all frames of a step must be on the host or all on the GPU")
-            if dev:
-                if frame.dtype != torch.uint8 or frame.dim() != 3 or frame.shape[2] != 3 or not frame.is_contiguous():
-                    raise RuntimeError("DiMPBatchTracker.step: a CUDA frame must be a contiguous uint8 [H,W,3] tensor")
-                ptr, H, W = frame.data_ptr(), frame.shape[0], frame.shape[1]
-            else:
-                buf, ptr = self._host_frame(slot, frame)
-                keep.append(buf)
-                H, W = buf.shape[0], buf.shape[1]
             it.slot, it.image, it.H, it.W = int(slot), ptr, int(H), int(W)
             it.init = int(init is not None)
             for i in range(4):

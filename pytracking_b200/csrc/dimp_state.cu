@@ -143,16 +143,6 @@ extern "C" int b200trk_dimp_localize_host(b200trk_dimp_state_t* s, const float* 
     return 0;
 }
 
-// Device half of DiMP.update_classifier shared by the host-buffer call below and by dimp_tracker.cu.
-int b200trk::dimp_state_update(b200trk_dimp_state* s, int scale_ind, int replace_ind, const float* target_box_host,
-                               const float* sample_weights_host, int n_stored, int num_iter, cudaStream_t st) {
-    B200_REQUIRE(s && target_box_host && sample_weights_host, "dimp_update: null pointer");
-    B200_REQUIRE(s->clf, "dimp_update: the state is a slot of a batch; its features are in the batch's buffer");
-    B200_REQUIRE(scale_ind >= 0 && scale_ind < s->max_batch, "dimp_update: scale_ind=%d", scale_ind);
-    return dimp_state_insert(s, s->clf + (size_t)s->Cc * s->Hc * s->Wc * scale_ind, replace_ind, target_box_host, sample_weights_host,
-                             n_stored, num_iter, st);
-}
-
 int b200trk::dimp_state_insert(b200trk_dimp_state* s, const float* feat, int replace_ind, const float* target_box_host,
                                const float* sample_weights_host, int n_stored, int num_iter, cudaStream_t st) {
     B200_REQUIRE(s && feat && target_box_host && sample_weights_host, "dimp_update: null pointer");
@@ -187,7 +177,12 @@ int b200trk::dimp_state_optimize(b200trk_dimp_state* s, int n_stored, int num_it
                               nullptr, nullptr, st);
 }
 
+// Device half of DiMP.update_classifier for the features of crop scale_ind of the last localize call
 extern "C" int b200trk_dimp_update_host(b200trk_dimp_state_t* s, int scale_ind, int replace_ind, const float* target_box_host,
                                         const float* sample_weights_host, int n_stored, int num_iter, b200trk_stream_t stream) {
-    return dimp_state_update(s, scale_ind, replace_ind, target_box_host, sample_weights_host, n_stored, num_iter, (cudaStream_t)stream);
+    B200_REQUIRE(s && target_box_host && sample_weights_host, "dimp_update: null pointer");
+    B200_REQUIRE(s->clf, "dimp_update: the state is a slot of a batch; its features are in the batch's buffer");
+    B200_REQUIRE(scale_ind >= 0 && scale_ind < s->max_batch, "dimp_update: scale_ind=%d", scale_ind);
+    return dimp_state_insert(s, s->clf + (size_t)s->Cc * s->Hc * s->Wc * scale_ind, replace_ind, target_box_host, sample_weights_host,
+                             n_stored, num_iter, (cudaStream_t)stream);
 }

@@ -39,10 +39,9 @@ int dimp_state_create_newton(b200trk_dimp_state** out, b200trk_net* net, int mem
                              float feat_stride, float step_length, float reg_weight, float alpha_eps, int has_softmax_reg,
                              float softmax_reg, float label_threshold, int normalize_label, float label_shrink, float uni_weight,
                              float* filter_ext);
-// dimp_state_update with the new sample's features given by pointer (device [C,H,W]) instead of a batch index into s->clf
+// The memory update of DiMP.update_classifier: the sample `feat` (device [C,H,W]) with its box goes to memory slot replace_ind, the
+// first n_stored sample weights are replaced, then num_iter optimiser iterations run (none for num_iter <= 0)
 int dimp_state_insert(b200trk_dimp_state* s, const float* feat, int replace_ind, const float* target_box_host,
-                      const float* sample_weights_host, int n_stored, int num_iter, cudaStream_t st);
-int dimp_state_update(b200trk_dimp_state* s, int scale_ind, int replace_ind, const float* target_box_host,
                       const float* sample_weights_host, int n_stored, int num_iter, cudaStream_t st);
 // num_iter iterations of the state's online optimiser over the first n_stored samples of its pitched memory, filter in place
 int dimp_state_optimize(b200trk_dimp_state* s, int n_stored, int num_iter, cudaStream_t st);

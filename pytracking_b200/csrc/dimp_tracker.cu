@@ -16,6 +16,7 @@
 #include "dimp_state.cuh"
 #include <algorithm>
 #include <cmath>
+#include <cstdio>
 #include <cstring>
 #include <limits>
 
@@ -26,6 +27,44 @@ using namespace b200trk;
 namespace {
 
 inline float f32(double x) { return (float)x; }
+
+// Host frames go up on a copy stream of their own: the previous frame's steepest-descent update may still be running on the caller's
+// stream (a frame call returns as soon as the box is known).  The device buffer is free to overwrite: the previous crop kernel finished
+// before the previous call returned, which synchronised on its localisation result.
+struct FrameUpload {
+    uint8_t* dev = nullptr; size_t cap = 0;
+    cudaStream_t stream = nullptr; cudaEvent_t ev = nullptr;
+
+    ~FrameUpload() {
+        if (dev) cudaFree(dev);
+        if (stream) cudaStreamDestroy(stream);
+        if (ev) cudaEventDestroy(ev);
+    }
+
+    // Copies the n uint8 [H[k],W[k],3] host frames im[k] to 256-byte-aligned offsets of `dev`, replaces each im[k] by its device copy
+    // and makes `st` wait for the copies.
+    int upload(int n, const uint8_t* im[], const int H[], const int W[], cudaStream_t st) {
+        size_t off[kBatchMax], total = 0;
+        for (int k = 0; k < n; ++k) { off[k] = total; total += ((size_t)H[k] * W[k] * 3 + 255) / 256 * 256; }
+        if (total > cap) {
+            if (dev) B200_CHECK_CUDA(cudaFree(dev));
+            dev = nullptr; cap = 0;
+            B200_CHECK_CUDA(cudaMalloc((void**)&dev, total));
+            cap = total;
+        }
+        if (!stream) {
+            B200_CHECK_CUDA(cudaStreamCreateWithFlags(&stream, cudaStreamNonBlocking));
+            B200_CHECK_CUDA(cudaEventCreateWithFlags(&ev, cudaEventDisableTiming));
+        }
+        for (int k = 0; k < n; ++k) {
+            B200_CHECK_CUDA(cudaMemcpyAsync(dev + off[k], im[k], (size_t)H[k] * W[k] * 3, cudaMemcpyHostToDevice, stream));
+            im[k] = dev + off[k];
+        }
+        B200_CHECK_CUDA(cudaEventRecord(ev, stream));
+        B200_CHECK_CUDA(cudaStreamWaitEvent(st, ev, 0));
+        return 0;
+    }
+};
 
 }  // namespace
 
@@ -51,9 +90,8 @@ struct b200trk_dimp_tracker {
     float pos_iounet[2] = {0, 0}; int has_pos_iounet = 0;
     std::vector<float> noise;                        // uniform numbers for the next frame's random proposals
     uint64_t rng = 0x9E3779B97F4A7C15ull;
-    // device side
-    cudaStream_t copy_stream = nullptr; cudaEvent_t ev_img = nullptr;   // frame upload overlaps the previous frame's filter update
-    uint8_t* img_dev = nullptr; size_t img_cap = 0;
+    // device side (a batch slot uses the batch's frames and results instead)
+    FrameUpload frames;
     b200trk_loc_result_t* loc_dev = nullptr;
     b200trk_loc_result_t* loc_host = nullptr;      // pinned
 };
@@ -163,8 +201,9 @@ extern "C" int b200trk_dimp_tracker_create(b200trk_dimp_tracker_t** out, b200trk
         t->feature_sz[0] = (float)state->Hc; t->feature_sz[1] = (float)state->Wc;
         t->kernel_size[0] = t->kernel_size[1] = (float)state->ksz;
         t->score_sz[0] = (float)state->Ho; t->score_sz[1] = (float)state->Wo;
-        if (cudaMalloc((void**)&t->loc_dev, sizeof(b200trk_loc_result_t)) != cudaSuccess ||
-            cudaMallocHost((void**)&t->loc_host, sizeof(b200trk_loc_result_t)) != cudaSuccess) {
+        // a state without per-frame buffers is a batch slot: the batch holds the localisation results of all its slots
+        if (state->clf && (cudaMalloc((void**)&t->loc_dev, sizeof(b200trk_loc_result_t)) != cudaSuccess ||
+                           cudaMallocHost((void**)&t->loc_host, sizeof(b200trk_loc_result_t)) != cudaSuccess)) {
             set_error("dimp_tracker_create: allocation failed");
             b200trk_dimp_tracker_destroy(t);
             return 1;
@@ -180,9 +219,6 @@ extern "C" int b200trk_dimp_tracker_create(b200trk_dimp_tracker_t** out, b200trk
 
 extern "C" int b200trk_dimp_tracker_destroy(b200trk_dimp_tracker_t* t) {
     if (!t) return 0;
-    if (t->img_dev) cudaFree(t->img_dev);
-    if (t->copy_stream) cudaStreamDestroy(t->copy_stream);
-    if (t->ev_img) cudaEventDestroy(t->ev_img);
     if (t->loc_dev) cudaFree(t->loc_dev);
     if (t->loc_host) cudaFreeHost(t->loc_host);
     for (float* q : {t->mod3, t->mod4, t->iou3, t->iou4, t->boxes_dev}) if (q) cudaFree(q);
@@ -513,13 +549,19 @@ extern "C" int b200trk_dimp_tracker_attach_iounet(b200trk_dimp_tracker_t* t, b20
 // ---------------------------------------------------------------------------------------------------------------------------
 // device launches
 // ---------------------------------------------------------------------------------------------------------------------------
+// A crop the sampling kernels can read: a decimation factor >= 1, a non-empty patch, and the win_h x win_w window inside the resampled patch
+static int crop_ok(const b200trk_crop_geom_t* g, int win_h, int win_w, const char* what) {
+    B200_REQUIRE(g->df >= 1 && g->in_h >= 1 && g->in_w >= 1 && g->out_h >= 1 && g->out_w >= 1, "%s: bad geometry", what);
+    B200_REQUIRE(g->win_r >= 0 && g->win_c >= 0 && g->win_r + win_h <= g->out_h && g->win_c + win_w <= g->out_w,
+                 "%s: window [%d+%d, %d+%d] outside the %dx%d resampled patch", what, g->win_r, win_h, g->win_c, win_w, g->out_h, g->out_w);
+    return 0;
+}
+
 extern "C" int b200trk_sample_patch(const uint8_t* image_dev, int H, int W, const b200trk_crop_geom_t* g, int win_h, int win_w, float* out,
                                     b200trk_stream_t stream) {
     B200_REQUIRE(image_dev && g && out, "sample_patch: null pointer");
-    B200_REQUIRE(H > 0 && W > 0 && win_h > 0 && win_w > 0 && g->df >= 1 && g->in_h >= 1 && g->in_w >= 1 && g->out_h >= 1 && g->out_w >= 1,
-                 "sample_patch: bad geometry");
-    B200_REQUIRE(g->win_r >= 0 && g->win_c >= 0 && g->win_r + win_h <= g->out_h && g->win_c + win_w <= g->out_w,
-                 "sample_patch: window [%d+%d, %d+%d] outside the %dx%d resampled patch", g->win_r, win_h, g->win_c, win_w, g->out_h, g->out_w);
+    B200_REQUIRE(H > 0 && W > 0 && win_h > 0 && win_w > 0, "sample_patch: bad geometry");
+    if (int e = crop_ok(g, win_h, win_w, "sample_patch")) return e;
     dim3 grid((win_w + 31) / 32, (win_h + 7) / 8);
     sample_patch_kernel<<<grid, 256, 0, (cudaStream_t)stream>>>(image_dev, H, W, *g, win_h, win_w, out);
     B200_LAUNCH_CHECK();
@@ -541,24 +583,21 @@ extern "C" int b200trk_dimp_localize(const float* scores, int S, int Ho, int Wo,
     return 0;
 }
 
-static int upload_image(b200trk_dimp_tracker* t, const uint8_t* image, int H, int W, cudaStream_t st) {
-    const size_t bytes = (size_t)H * W * 3;
-    if (bytes > t->img_cap) {
-        if (t->img_dev) B200_CHECK_CUDA(cudaFree(t->img_dev));
-        t->img_dev = nullptr; t->img_cap = 0;
-        B200_CHECK_CUDA(cudaMalloc((void**)&t->img_dev, bytes));
-        t->img_cap = bytes;
-    }
-    // The previous frame's steepest-descent update may still be running on `st` (track returns as soon as the box is known); the
-    // frame travels on a copy stream of its own meanwhile. (The device image is free: the previous crop kernel finished before the
-    // previous call returned, which synchronised on its localisation result.)
-    if (!t->copy_stream) {
-        B200_CHECK_CUDA(cudaStreamCreateWithFlags(&t->copy_stream, cudaStreamNonBlocking));
-        B200_CHECK_CUDA(cudaEventCreateWithFlags(&t->ev_img, cudaEventDisableTiming));
-    }
-    B200_CHECK_CUDA(cudaMemcpyAsync(t->img_dev, image, bytes, cudaMemcpyHostToDevice, t->copy_stream));
-    B200_CHECK_CUDA(cudaEventRecord(t->ev_img, t->copy_stream));
-    B200_CHECK_CUDA(cudaStreamWaitEvent(st, t->ev_img, 0));
+// The device half of initialize (dimp.py:601-602, FilterInitializerZero): the first frame's features `feat` become sample 0 with box
+// `box`, and num_iter iterations run from the zero filter.  The reference passes sample_weight = None, which both optimisers read as
+// 1/num_images (optimizer.py:122-123 GN, :387-388 Newton): with one sample that is the weight 1 uploaded here.
+static int first_frame_update(b200trk_dimp_state* s, const float* feat, const float box[4], int num_iter, cudaStream_t st) {
+    B200_CHECK_CUDA(cudaMemsetAsync(s->filter, 0, (size_t)s->Cc * s->ksz * s->ksz * sizeof(float), st));
+    B200_CHECK_CUDA(cudaMemsetAsync(s->sw, 0, (size_t)s->memory_size * sizeof(float), st));
+    const float one = 1.f;
+    return dimp_state_insert(s, feat, 0, box, &one, 1, num_iter, st);
+}
+
+// The device half of update_classifier (dimp.py:605-625) after a frame's commit: store the sample `feat` and optimise, or only optimise
+// (update_classifier can run iterations without storing a sample: train_sample_interval > 1)
+static int frame_update(b200trk_dimp_tracker* t, const float* feat, const b200trk_frame_info_t* info, cudaStream_t st) {
+    if (info->updated) return dimp_state_insert(t->st, feat, info->replace_ind, info->target_box, t->sw.data(), info->n_stored, info->num_iter, st);
+    if (info->num_iter > 0) return dimp_state_optimize(t->st, info->n_stored, info->num_iter, st);
     return 0;
 }
 
@@ -570,17 +609,11 @@ extern "C" int b200trk_dimp_tracker_initialize_host(b200trk_dimp_tracker_t* t, c
     b200trk_dimp_state* s = t->st;
     b200trk_crop_geom_t g; float box[4];
     if (int e = b200trk_dimp_tracker_init_state(t, H, W, init_bbox, &g, box)) return e;
-    if (int e = upload_image(t, image, H, W, st)) return e;
+    if (int e = t->frames.upload(1, &image, &H, &W, st)) return e;
     const int iss = t->p.image_sample_size;
-    if (int e = b200trk_sample_patch(t->img_dev, H, W, &g, iss, iss, s->crop, stream)) return e;
+    if (int e = b200trk_sample_patch(image, H, W, &g, iss, iss, s->crop, stream)) return e;
     if (int e = b200trk_net_forward(s->net, s->crop, 1, nullptr, nullptr, s->clf, stream)) return e;
-    // FilterInitializerZero (dimp.py:601-602) + net_opt_iter iterations on the single init sample. The reference passes
-    // sample_weight = None, which both optimisers read as 1/num_images (optimizer.py:122-123 GN, :387-388 Newton): with one sample
-    // that is the weight 1 uploaded here.
-    B200_CHECK_CUDA(cudaMemsetAsync(s->filter, 0, (size_t)s->Cc * s->ksz * s->ksz * sizeof(float), st));
-    B200_CHECK_CUDA(cudaMemsetAsync(s->sw, 0, (size_t)s->memory_size * sizeof(float), st));
-    const float one = 1.f;
-    if (int e = dimp_state_update(s, 0, 0, box, &one, 1, t->p.net_opt_iter > 0 ? t->p.net_opt_iter : 0, st)) return e;
+    if (int e = first_frame_update(s, s->clf, box, t->p.net_opt_iter > 0 ? t->p.net_opt_iter : 0, st)) return e;
     B200_CHECK_CUDA(cudaStreamSynchronize(st));
     return 0;
 }
@@ -594,20 +627,26 @@ static void loc_inputs(const b200trk_dimp_tracker* t, const b200trk_crop_geom_t&
     }
 }
 
+// The refusals of a frame of a running sequence: the tracker holds one, and the frame has the size of the sequence's first frame
+static int tracking_ok(const b200trk_dimp_tracker* t, int H, int W, const char* what) {
+    B200_REQUIRE(t->initialized, "%s: not tracking a sequence (never initialised, or released)", what);
+    B200_REQUIRE((float)H == t->image_sz[0] && (float)W == t->image_sz[1], "%s: frame is %dx%d, the sequence started with %dx%d", what, H, W,
+                 (int)t->image_sz[0], (int)t->image_sz[1]);
+    return 0;
+}
+
 static int track_frame(b200trk_dimp_tracker* t, const uint8_t* image, bool on_device, int H, int W, b200trk_frame_info_t* info,
                        b200trk_stream_t stream) {
     B200_REQUIRE(t && image && info, "dimp_track_host: null pointer");
     B200_REQUIRE(t->st, "dimp_track_host: host-logic-only tracker (created without a device state)");
-    B200_REQUIRE(t->initialized, "dimp_track_host: tracker not initialised");
-    B200_REQUIRE((float)H == t->image_sz[0] && (float)W == t->image_sz[1], "dimp_track_host: frame is %dx%d, the sequence started with %dx%d",
-                 H, W, (int)t->image_sz[0], (int)t->image_sz[1]);
+    if (int e = tracking_ok(t, H, W, "dimp_track_host")) return e;
     cudaStream_t st = (cudaStream_t)stream;
     b200trk_dimp_state* s = t->st;
     b200trk_crop_geom_t g;
     if (int e = b200trk_dimp_tracker_plan_crop(t, &g)) return e;
-    if (!on_device) { if (int e = upload_image(t, image, H, W, st)) return e; }
+    if (!on_device) { if (int e = t->frames.upload(1, &image, &H, &W, st)) return e; }
     const int iss = t->p.image_sample_size;
-    if (int e = b200trk_sample_patch(on_device ? image : t->img_dev, H, W, &g, iss, iss, s->crop, stream)) return e;
+    if (int e = b200trk_sample_patch(image, H, W, &g, iss, iss, s->crop, stream)) return e;
     if (int e = b200trk_net_forward(s->net, s->crop, 1, nullptr, nullptr, s->clf, stream)) return e;
     if (int e = b200trk_apply_filter(s->clf, s->filter, s->scores, 1, s->Cc, s->Hc, s->Wc, s->ksz, nullptr, nullptr, stream)) return e;
     float neigh[2], pv[2];
@@ -631,13 +670,7 @@ static int track_frame(b200trk_dimp_tracker* t, const uint8_t* image, bool on_de
         if (int e = b200trk_dimp_tracker_commit_refine(t, &g, t->boxes_host, t->boxes_host + 64, R, info)) return e;
     }
     if (int e = b200trk_dimp_tracker_commit_update(t, &g, info, nullptr)) return e;
-    if (info->updated) {
-        if (int e = dimp_state_update(s, 0, info->replace_ind, info->target_box, t->sw.data(), info->n_stored, info->num_iter, st)) return e;
-    } else if (info->num_iter > 0) {
-        // update_classifier can optimise without storing a sample (train_sample_interval > 1): run the iterations only
-        if (int e = dimp_state_optimize(s, info->n_stored, info->num_iter, st)) return e;
-    }
-    return 0;
+    return frame_update(t, s->clf, info, st);
 }
 
 extern "C" int b200trk_dimp_track_host(b200trk_dimp_tracker_t* t, const uint8_t* image, int H, int W, b200trk_frame_info_t* info,
@@ -661,25 +694,23 @@ struct b200trk_dimp_batch {
     b200trk_net* net = nullptr;
     int cap = 0, Cc = 0, Hc = 0, Wc = 0, Ho = 0, Wo = 0, ksz = 4, iss = 0;
     b200trk_dimp_params_t p;
-    b200trk_dimp_tracker* t[kBatchMax] = {};
-    b200trk_dimp_state* st[kBatchMax] = {};
+    b200trk_dimp_tracker* t[kBatchMax] = {};                                         // the slots; the batch also owns their states t[i]->st
     float *crop = nullptr, *clf = nullptr, *scores = nullptr, *filters = nullptr;   // device [S,3,iss,iss] [S,C,Hc,Wc] [S,Ho,Wo] [S,C,k,k]
-    uint8_t* img_dev = nullptr; size_t img_cap = 0;                                  // the step's uploaded frames, back to back
-    cudaStream_t copy_stream = nullptr; cudaEvent_t ev_img = nullptr;
+    FrameUpload frames;                                                              // the step's host frames, back to back
     b200trk_loc_result_t* loc_dev = nullptr;                                         // [S]
     b200trk_loc_result_t* loc_host = nullptr;                                        // pinned [S]
 };
 
 extern "C" int b200trk_dimp_batch_destroy(b200trk_dimp_batch_t* b) {
     if (!b) return 0;
-    for (int i = 0; i < kBatchMax; ++i) {
-        if (b->t[i]) b200trk_dimp_tracker_destroy(b->t[i]);
-        if (b->st[i]) b200trk_dimp_state_destroy(b->st[i]);
+    for (b200trk_dimp_tracker* t : b->t) {
+        if (!t) continue;
+        b200trk_dimp_state* s = t->st;
+        b200trk_dimp_tracker_destroy(t);
+        b200trk_dimp_state_destroy(s);
     }
-    for (void* q : {(void*)b->crop, (void*)b->clf, (void*)b->scores, (void*)b->filters, (void*)b->img_dev, (void*)b->loc_dev}) if (q) cudaFree(q);
+    for (void* q : {(void*)b->crop, (void*)b->clf, (void*)b->scores, (void*)b->filters, (void*)b->loc_dev}) if (q) cudaFree(q);
     if (b->loc_host) cudaFreeHost(b->loc_host);
-    if (b->copy_stream) cudaStreamDestroy(b->copy_stream);
-    if (b->ev_img) cudaEventDestroy(b->ev_img);
     delete b;
     return 0;
 }
@@ -707,15 +738,14 @@ static int batch_create(b200trk_dimp_batch** out, b200trk_net* net, int capacity
     if (!alloc((void**)&b->crop, S * 3 * net->crop_h * net->crop_w * sizeof(float)) ||
         !alloc((void**)&b->clf, S * b->Cc * b->Hc * b->Wc * sizeof(float)) || !alloc((void**)&b->scores, S * b->Ho * b->Wo * sizeof(float)) ||
         !alloc((void**)&b->filters, S * fsz * sizeof(float)) || !alloc((void**)&b->loc_dev, S * sizeof(b200trk_loc_result_t)) ||
-        cudaMallocHost((void**)&b->loc_host, S * sizeof(b200trk_loc_result_t)) != cudaSuccess ||
-        cudaStreamCreateWithFlags(&b->copy_stream, cudaStreamNonBlocking) != cudaSuccess ||
-        cudaEventCreateWithFlags(&b->ev_img, cudaEventDisableTiming) != cudaSuccess) {
+        cudaMallocHost((void**)&b->loc_host, S * sizeof(b200trk_loc_result_t)) != cudaSuccess) {
         set_error("dimp_batch_create: allocation failed");
         return fail(1);
     }
     for (int i = 0; i < capacity; ++i) {
-        if (int e = make_state(b->filters + i * fsz, &b->st[i])) return fail(e);
-        if (int e = b200trk_dimp_tracker_create(&b->t[i], b->st[i], params)) return fail(e);
+        b200trk_dimp_state* s = nullptr;
+        if (int e = make_state(b->filters + i * fsz, &s)) return fail(e);
+        if (int e = b200trk_dimp_tracker_create(&b->t[i], s, params)) { b200trk_dimp_state_destroy(s); return fail(e); }
     }
     *out = b;
     return 0;
@@ -775,56 +805,34 @@ static int batch_step(b200trk_dimp_batch* b, const b200trk_batch_item_t* items, 
     B200_REQUIRE(n >= 1 && n <= b->cap, "dimp_batch_step: %d items for a batch of %d slots", n, b->cap);
     // every refusal before any state changes
     bool seen[kBatchMax] = {};
+    char what[kBatchMax][40];                                                        // "dimp_batch_step: slot %d", the refusals' prefix
     for (int k = 0; k < n; ++k) {
         const b200trk_batch_item_t& it = items[k];
         B200_REQUIRE(it.slot >= 0 && it.slot < b->cap, "dimp_batch_step: slot %d outside 0..%d", it.slot, b->cap - 1);
         B200_REQUIRE(!seen[it.slot], "dimp_batch_step: slot %d appears twice in one step", it.slot);
         seen[it.slot] = true;
-        B200_REQUIRE(it.image && it.H > 0 && it.W > 0, "dimp_batch_step: slot %d: no frame or an empty one (%dx%d)", it.slot, it.H, it.W);
-        const b200trk_dimp_tracker* t = b->t[it.slot];
+        std::snprintf(what[k], sizeof(what[k]), "dimp_batch_step: slot %d", it.slot);
+        B200_REQUIRE(it.image && it.H > 0 && it.W > 0, "%s: no frame or an empty one (%dx%d)", what[k], it.H, it.W);
         if (it.init) {
-            B200_REQUIRE(it.init_bbox[2] > 0 && it.init_bbox[3] > 0, "dimp_batch_step: slot %d: init box of size %gx%g", it.slot,
-                         it.init_bbox[2], it.init_bbox[3]);
-        } else {
-            B200_REQUIRE(t->initialized, "dimp_batch_step: slot %d is not tracking a sequence (never initialised, or released)", it.slot);
-            B200_REQUIRE((float)it.H == t->image_sz[0] && (float)it.W == t->image_sz[1],
-                         "dimp_batch_step: slot %d: frame is %dx%d, its sequence started with %dx%d", it.slot, it.H, it.W,
-                         (int)t->image_sz[0], (int)t->image_sz[1]);
+            B200_REQUIRE(it.init_bbox[2] > 0 && it.init_bbox[3] > 0, "%s: init box of size %gx%g", what[k], it.init_bbox[2], it.init_bbox[3]);
+        } else if (int e = tracking_ok(b->t[it.slot], it.H, it.W, what[k])) {
+            return e;
         }
     }
     cudaStream_t st = (cudaStream_t)stream;
     const int iss = b->iss;
     // 1. crop plans on the host
-    b200trk_crop_geom_t g[kBatchMax];
+    SampleBatchArgs sa;
     float box[kBatchMax][4];
     for (int k = 0; k < n; ++k) {
         const b200trk_batch_item_t& it = items[k];
-        if (it.init) { if (int e = b200trk_dimp_tracker_init_state(b->t[it.slot], it.H, it.W, it.init_bbox, &g[k], box[k])) return e; }
-        else if (int e = b200trk_dimp_tracker_plan_crop(b->t[it.slot], &g[k])) return e;
-        B200_REQUIRE(g[k].win_r >= 0 && g[k].win_c >= 0 && g[k].win_r + iss <= g[k].out_h && g[k].win_c + iss <= g[k].out_w && g[k].df >= 1 &&
-                     g[k].in_h >= 1 && g[k].in_w >= 1, "dimp_batch_step: slot %d: bad crop geometry", it.slot);
+        if (it.init) { if (int e = b200trk_dimp_tracker_init_state(b->t[it.slot], it.H, it.W, it.init_bbox, &sa.g[k], box[k])) return e; }
+        else if (int e = b200trk_dimp_tracker_plan_crop(b->t[it.slot], &sa.g[k])) return e;
+        if (int e = crop_ok(&sa.g[k], iss, iss, what[k])) return e;
+        sa.im[k] = it.image; sa.H[k] = it.H; sa.W[k] = it.W; sa.dst[k] = it.slot;
     }
-    // 2. the frames, on the copy stream behind one event (the previous step's crop kernel finished before it returned)
-    SampleBatchArgs sa;
-    size_t off[kBatchMax], total = 0;
-    for (int k = 0; k < n; ++k) { off[k] = total; total += ((size_t)items[k].H * items[k].W * 3 + 255) / 256 * 256; }
-    if (!on_device) {
-        if (total > b->img_cap) {
-            if (b->img_dev) B200_CHECK_CUDA(cudaFree(b->img_dev));
-            b->img_dev = nullptr; b->img_cap = 0;
-            B200_CHECK_CUDA(cudaMalloc((void**)&b->img_dev, total));
-            b->img_cap = total;
-        }
-        for (int k = 0; k < n; ++k)
-            B200_CHECK_CUDA(cudaMemcpyAsync(b->img_dev + off[k], items[k].image, (size_t)items[k].H * items[k].W * 3, cudaMemcpyHostToDevice,
-                                            b->copy_stream));
-        B200_CHECK_CUDA(cudaEventRecord(b->ev_img, b->copy_stream));
-        B200_CHECK_CUDA(cudaStreamWaitEvent(st, b->ev_img, 0));
-    }
-    for (int k = 0; k < n; ++k) {
-        sa.im[k] = on_device ? items[k].image : b->img_dev + off[k];
-        sa.H[k] = items[k].H; sa.W[k] = items[k].W; sa.dst[k] = items[k].slot; sa.g[k] = g[k];
-    }
+    // 2. the frames, on the copy stream behind one event
+    if (!on_device) { if (int e = b->frames.upload(n, sa.im, sa.H, sa.W, st)) return e; }
     // 3. one crop launch for every item
     sample_patch_batch_kernel<<<dim3((iss + 31) / 32, (iss + 7) / 8, n), 256, 0, st>>>(sa, iss, b->crop);
     B200_LAUNCH_CHECK();
@@ -857,7 +865,7 @@ static int batch_step(b200trk_dimp_batch* b, const b200trk_batch_item_t* items, 
     for (int k = 0; k < n; ++k) {
         if (items[k].init) continue;
         la.slot[nt] = items[k].slot;
-        loc_inputs(b->t[items[k].slot], g[k], la.neigh[nt], la.prev_vec[nt]);
+        loc_inputs(b->t[items[k].slot], sa.g[k], la.neigh[nt], la.prev_vec[nt]);
         tracked[nt++] = k;
     }
     if (nt > 0) {
@@ -873,30 +881,19 @@ static int batch_step(b200trk_dimp_batch* b, const b200trk_batch_item_t* items, 
     for (int j = 0; j < nt; ++j) {
         const int k = tracked[j], slot = items[k].slot;
         b200trk_dimp_tracker* t = b->t[slot];
-        b200trk_frame_info_t* info = &infos[k];
-        if (int e = b200trk_dimp_tracker_commit_localize(t, &g[k], &b->loc_host[j], info)) return e;
-        if (int e = b200trk_dimp_tracker_commit_update(t, &g[k], info, nullptr)) return e;
-        if (info->updated) {
-            if (int e = dimp_state_insert(b->st[slot], b->clf + plane * slot, info->replace_ind, info->target_box, t->sw.data(), info->n_stored,
-                                          info->num_iter, st)) return e;
-        } else if (info->num_iter > 0) {
-            if (int e = dimp_state_optimize(b->st[slot], info->n_stored, info->num_iter, st)) return e;
-        }
+        if (int e = b200trk_dimp_tracker_commit(t, &sa.g[k], &b->loc_host[j], &infos[k], nullptr)) return e;
+        if (int e = frame_update(t, b->clf + plane * slot, &infos[k], st)) return e;
     }
-    // initialisation (b200trk_dimp_tracker_initialize_host): net_opt_iter iterations from the zero filter on the one init sample
+    // initialisation, as b200trk_dimp_tracker_initialize_host
     for (int k = 0; k < n; ++k) {
         if (!items[k].init) continue;
         const int slot = items[k].slot;
-        b200trk_dimp_state* s = b->st[slot];
         b200trk_frame_info_t* info = &infos[k];
         std::memset(info, 0, sizeof(*info));
-        info->crop = g[k];
+        info->crop = sa.g[k];
         for (int i = 0; i < 4; ++i) { info->bbox[i] = f32(items[k].init_bbox[i]); info->target_box[i] = box[k][i]; }
         info->updated = 1; info->n_stored = 1; info->num_iter = b->p.net_opt_iter > 0 ? b->p.net_opt_iter : 0;
-        B200_CHECK_CUDA(cudaMemsetAsync(s->filter, 0, (size_t)s->Cc * s->ksz * s->ksz * sizeof(float), st));
-        B200_CHECK_CUDA(cudaMemsetAsync(s->sw, 0, (size_t)s->memory_size * sizeof(float), st));
-        const float one = 1.f;
-        if (int e = dimp_state_insert(s, b->clf + plane * slot, 0, box[k], &one, 1, info->num_iter, st)) return e;
+        if (int e = first_frame_update(b->t[slot]->st, b->clf + plane * slot, box[k], info->num_iter, st)) return e;
     }
     return 0;
 }

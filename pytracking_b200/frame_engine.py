@@ -92,40 +92,45 @@ def newton_scalars(state_dict, nw):
     return float(torch.exp(log_step).item()), float((freg * freg).clamp(min=nw["min_filter_reg"] ** 2).item())
 
 
+def optimizer_args(state_dict, newton):
+    """The online optimiser's arguments after `filter_size` of b200trk_dimp_state_create / b200trk_dimp_batch_create (newton=None:
+    DiMPSteepestDescentGN over the state_dict's three LUTs) or of b200trk_prdimp_state_create / b200trk_prdimp_batch_create (newton:
+    PrDiMPSteepestDescentNewton arguments as newton_hparams returns them), followed by the optimiser's step_length and reg_weight.
+    The GN optimiser's bin_displacement, feat_stride, min_filter_reg and alpha_eps are DiMP-50's 0.1, 16, 1e-3 and 0."""
+    po = "classifier.filter_optimizer."
+    if newton is None:
+        luts = [state_dict[po + k].detach().float().reshape(-1).cpu().numpy() for k in
+                ("label_map_predictor.weight", "target_mask_predictor.0.weight", "spatial_weight_predictor.weight")]
+        step_length = float(torch.exp(state_dict[po + "log_step_length"].float()).item())
+        reg_weight = max(float(state_dict[po + "filter_reg"].float().item()) ** 2, 1e-3 ** 2)
+        args = [(C.c_float * t.size).from_buffer_copy(t) for t in luts] + [luts[0].size, 0.1, 16.0, step_length, reg_weight, 0.0]
+    else:
+        step_length, reg_weight = newton_scalars(state_dict, newton)
+        sreg = newton["softmax_reg"]
+        args = [float(newton["gauss_sigma"]), float(newton["feat_stride"]), step_length, reg_weight, float(newton["alpha_eps"]),
+                int(sreg is not None), 0.0 if sreg is None else float(sreg), float(newton["label_threshold"]),
+                int(bool(newton["normalize_label"])), float(newton["label_shrink"]), float(newton["init_uni_weight"] or 0.0)]
+    return args, step_length, reg_weight
+
+
 class DiMPFrameEngine:
-    def __init__(self, state_dict, arch="resnet50", filter_size=4, memory_size=50, max_batch=1, crop_size=288,
-                 precision=0, alpha_eps=0.0, min_filter_reg=1e-3, bin_displacement=0.1, feat_stride=16.0, device=None, newton=None):
+    def __init__(self, state_dict, arch="resnet50", filter_size=4, memory_size=50, max_batch=1, crop_size=288, precision=0, device=None,
+                 newton=None):
         """newton: None for DiMP (DiMPSteepestDescentGN over the three LUTs of the state_dict), or a dict of
         PrDiMPSteepestDescentNewton constructor arguments (tracker.NEWTON_DEFAULTS names) for PrDiMP; the GN keys are then not read.
         A state_dict that carries the optimiser's learnt log_step_length / filter_reg (a trained PrDiMP net) supplies those two."""
         self.backbone = BackboneEngine(state_dict, arch, filter_size, max_batch, crop_size, precision, device)
         self.device = self.backbone.device
-        po = "classifier.filter_optimizer."
         self.memory_size, self.filter_size, self.max_batch = memory_size, filter_size, max_batch
-        self.newton = None
-        h = C.c_void_p()
-        if newton is None:
-            luts = [state_dict[po + k].detach().float().reshape(-1).contiguous().cpu() for k in
-                    ("label_map_predictor.weight", "target_mask_predictor.0.weight", "spatial_weight_predictor.weight")]
-            self.step_length = float(torch.exp(state_dict[po + "log_step_length"].float()).item())
-            self.reg_weight = max(float(state_dict[po + "filter_reg"].float().item()) ** 2, min_filter_reg ** 2)
-            with torch.cuda.device(self.device):
-                _lib.check(_lib.lib().b200trk_dimp_state_create(
-                    C.byref(h), self.backbone.handle, memory_size, filter_size, C.c_void_p(luts[0].data_ptr()),
-                    C.c_void_p(luts[1].data_ptr()), C.c_void_p(luts[2].data_ptr()), luts[0].numel(), bin_displacement,
-                    feat_stride, self.step_length, self.reg_weight, alpha_eps), "dimp_state_create")
-        else:
+        if newton is not None:
             from .tracker import newton_hparams
-            nw = newton_hparams(newton)
-            self.step_length, self.reg_weight = newton_scalars(state_dict, nw)
-            self.newton = nw
-            sreg = nw["softmax_reg"]
-            with torch.cuda.device(self.device):
-                _lib.check(_lib.lib().b200trk_prdimp_state_create(
-                    C.byref(h), self.backbone.handle, memory_size, filter_size, float(nw["gauss_sigma"]), float(nw["feat_stride"]),
-                    self.step_length, self.reg_weight, float(nw["alpha_eps"]), int(sreg is not None), 0.0 if sreg is None else float(sreg),
-                    float(nw["label_threshold"]), int(bool(nw["normalize_label"])), float(nw["label_shrink"]),
-                    float(nw["init_uni_weight"] or 0.0)), "prdimp_state_create")
+            newton = newton_hparams(newton)
+        self.newton = newton
+        args, self.step_length, self.reg_weight = optimizer_args(state_dict, newton)
+        create = "dimp_state_create" if newton is None else "prdimp_state_create"
+        h = C.c_void_p()
+        with torch.cuda.device(self.device):
+            _lib.check(getattr(_lib.lib(), "b200trk_" + create)(C.byref(h), self.backbone.handle, memory_size, filter_size, *args), create)
         self.state = h
         L = _lib.lib()
         cc, hc, wc = self.backbone.dims[6:9]

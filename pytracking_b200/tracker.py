@@ -109,6 +109,38 @@ def make_params(source=None, **overrides):
     return p
 
 
+def tracker_settings(params, newton, **param_overrides):
+    """(b200trk_dimp_params_t, Newton hyper-parameters or None) of a tracker.  `params`: a DimpParams, used as it is, or a
+    `TrackerParams` source for make_params.  For PrDiMP (`newton` a dict) the params' filter_reg / softmax_reg / label_threshold /
+    label_shrink apply to the optimiser (newton_hparams), and the localisation's softmax uses the optimiser's softmax_reg, as
+    localize_target does (dimp.py:207)."""
+    own = isinstance(params, _lib.DimpParams)
+    p = params if own else make_params(params, **param_overrides)
+    if newton is not None:
+        newton = newton_hparams(newton, None if own else params, **param_overrides)
+        p.has_softmax_reg = int(newton["softmax_reg"] is not None)
+        p.softmax_reg = 0.0 if newton["softmax_reg"] is None else float(newton["softmax_reg"])
+    return p, newton
+
+
+def frame_pointer(image, staging, key, who):
+    """A uint8 [H,W,3] RGB frame -> (keep-alive, pointer, H, W, on_device).  A CUDA tensor or a pinned host tensor is used in place.
+    Any other frame (ndarray, pageable tensor) is copied into the pinned buffer staging[key], which is reused while the frame size
+    stays the same; the library then uploads it with one asynchronous copy."""
+    if isinstance(image, torch.Tensor) and (image.is_cuda or image.is_pinned()):
+        if image.dtype != torch.uint8 or image.dim() != 3 or image.shape[2] != 3 or not image.is_contiguous():
+            raise RuntimeError("%s: a frame tensor must be contiguous uint8 [H,W,3], got %s %s" % (who, image.dtype, tuple(image.shape)))
+        return image, image.data_ptr(), int(image.shape[0]), int(image.shape[1]), image.is_cuda
+    a = np.ascontiguousarray(image)
+    if a.dtype != np.uint8 or a.ndim != 3 or a.shape[2] != 3:
+        raise RuntimeError("%s: a frame must be uint8 [H,W,3] (RGB), got %s %s" % (who, a.dtype, a.shape))
+    buf = staging.get(key)
+    if buf is None or tuple(buf.shape) != a.shape:
+        buf = staging[key] = torch.empty(a.shape, dtype=torch.uint8).pin_memory()
+    buf.numpy()[...] = a
+    return buf, buf.data_ptr(), a.shape[0], a.shape[1], False
+
+
 class HostLogic:
     """The host half of the tracker alone (no GPU): crop planning and the post-localisation state update.  Used by the CPU tests."""
 
@@ -168,13 +200,8 @@ class DiMPTracker(HostLogic):
     softmax then uses the optimiser's softmax_reg, as localize_target does (dimp.py:207)."""
 
     def __init__(self, state_dict, params=None, arch="resnet50", precision=0, device=None, newton=None, **param_overrides):
-        self.params = params if isinstance(params, _lib.DimpParams) else make_params(params, **param_overrides)
+        self.params, newton = tracker_settings(params, newton, **param_overrides)
         p = self.params
-        if newton is not None:
-            src = None if isinstance(params, _lib.DimpParams) else params
-            newton = newton_hparams(newton, src, **param_overrides)
-            p.has_softmax_reg = int(newton["softmax_reg"] is not None)
-            p.softmax_reg = 0.0 if newton["softmax_reg"] is None else float(newton["softmax_reg"])
         self.engine = DiMPFrameEngine(state_dict, arch=arch, filter_size=4, memory_size=p.sample_memory_size, max_batch=1,
                                       crop_size=p.image_sample_size, precision=precision, device=device, newton=newton)
         self.device = self.engine.device
@@ -184,29 +211,22 @@ class DiMPTracker(HostLogic):
         self.handle = h
         self.info = _lib.FrameInfo()
         self.debug_info = {}
-        self._pinned = None
+        self._pinned = {}
         self.iou = None
         self.torch_noise = False       # True: draw the random proposals' noise with torch.rand, exactly where the reference does
 
     def _stream(self):
         return C.c_void_p(torch.cuda.current_stream(self.device).cuda_stream)
 
-    def _image(self, image):
-        if isinstance(image, torch.Tensor):                     # a pinned uint8 [H,W,3] tensor is used in place
-            if image.dtype != torch.uint8 or image.dim() != 3 or image.shape[2] != 3 or image.is_cuda or not image.is_contiguous():
-                raise RuntimeError("DiMPTracker: image must be a contiguous uint8 [H,W,3] host tensor or ndarray")
-            return image, image.data_ptr(), image.shape[0], image.shape[1]
-        a = np.ascontiguousarray(image)
-        if a.dtype != np.uint8 or a.ndim != 3 or a.shape[2] != 3:
-            raise RuntimeError("DiMPTracker: image must be uint8 [H,W,3] (RGB), got %s %s" % (a.dtype, a.shape))
-        if self._pinned is None or tuple(self._pinned.shape) != a.shape:
-            self._pinned = torch.empty(a.shape, dtype=torch.uint8).pin_memory()
-        self._pinned.numpy()[...] = a                            # pageable -> pinned staging, then one asynchronous H2D in the library
-        return self._pinned, self._pinned.data_ptr(), a.shape[0], a.shape[1]
+    def _frame(self, image, on_device):
+        keep, ptr, H, W, dev = frame_pointer(image, self._pinned, 0, "DiMPTracker")
+        if dev != on_device:
+            raise RuntimeError("DiMPTracker: this call takes a frame %s" % ("on the GPU" if on_device else "on the host"))
+        return keep, ptr, H, W
 
     def initialize(self, image, info):
         """DiMP.initialize for the un-augmented configuration (see b200trk_dimp_tracker_initialize_host)."""
-        keep, ptr, H, W = self._image(image)
+        keep, ptr, H, W = self._frame(image, False)
         bb = (C.c_double * 4)(*[float(v) for v in info["init_bbox"]])
         with torch.cuda.device(self.device):
             _lib.check(_lib.lib().b200trk_dimp_tracker_initialize_host(self.handle, C.c_void_p(ptr), H, W, C.byref(bb), self._stream()),
@@ -274,7 +294,7 @@ class DiMPTracker(HostLogic):
 
     def track(self, image, info=None):
         self._noise()
-        keep, ptr, H, W = self._image(image)
+        keep, ptr, H, W = self._frame(image, False)
         with torch.cuda.device(self.device):
             _lib.check(_lib.lib().b200trk_dimp_track_host(self.handle, C.c_void_p(ptr), H, W, C.byref(self.info), self._stream()),
                        "dimp_track_host")
@@ -285,11 +305,10 @@ class DiMPTracker(HostLogic):
     def track_device(self, image_dev):
         """`track` with the uint8 [H,W,3] frame already on the GPU (a CUDA tensor)."""
         self._noise()
-        if not image_dev.is_cuda or image_dev.dtype != torch.uint8 or image_dev.dim() != 3 or not image_dev.is_contiguous():
-            raise RuntimeError("DiMPTracker.track_device: contiguous uint8 [H,W,3] CUDA tensor")
+        keep, ptr, H, W = self._frame(image_dev, True)
         with torch.cuda.device(self.device):
-            _lib.check(_lib.lib().b200trk_dimp_track_device(self.handle, C.c_void_p(image_dev.data_ptr()), image_dev.shape[0],
-                                                            image_dev.shape[1], C.byref(self.info), self._stream()), "dimp_track_device")
+            _lib.check(_lib.lib().b200trk_dimp_track_device(self.handle, C.c_void_p(ptr), H, W, C.byref(self.info), self._stream()),
+                       "dimp_track_device")
         return self.info
 
     def close(self):
