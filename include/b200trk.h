@@ -289,6 +289,9 @@ int b200trk_net_op_output(const b200trk_net_t* net, int index, int S, float* dst
  * split-K arrivals complete, epilogue done), NULL detaches; and query the launch geometry {grid.x, grid.y, grid.z, BN}. */
 int b200trk_net_op_set_timing_buffer(b200trk_net_t* net, int index, unsigned long long* buf);
 int b200trk_net_op_grid(const b200trk_net_t* net, int index, int dims[4]);
+/* How that launch reduces its split-K partials: *mode = 0 no split-K, 1 through a thread-block cluster's distributed shared memory,
+ * 2 through the L2 workspace (more than 8 splits, or a cluster grid the device cannot hold at once). */
+int b200trk_net_op_splitk_reduction(const b200trk_net_t* net, int index, int* mode);
 
 /* ------------------------------------------------------------------------------------------------
  * ToMP model predictor core -- Transformer.forward

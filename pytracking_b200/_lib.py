@@ -132,6 +132,7 @@ SIGNATURES = {
     "b200trk_net_op_output": (_I, [_VP, _I, _I, _VP, _VP]),
     "b200trk_net_op_set_timing_buffer": (_I, [_VP, _I, _VP]),
     "b200trk_net_op_grid": (_I, [_VP, _I, C.POINTER(C.c_int * 4)]),
+    "b200trk_net_op_splitk_reduction": (_I, [_VP, _I, C.POINTER(C.c_int)]),
     "b200trk_transformer_create": (_I, [C.POINTER(_VP), C.POINTER(EncLayer), _I, C.POINTER(DecLayer), _I, _VP, _VP, _I, _I, _I, _I, _I]),
     "b200trk_transformer_destroy": (_I, [_VP]),
     "b200trk_transformer_forward": (_I, [_VP, _VP, _VP, _I, _VP, _VP, _VP, _VP, _VP]),

@@ -633,5 +633,9 @@ int tc_conv_grid(const Op& op, int dims[4]) {
     dims[0] = P.tiles_w * P.tiles_h * S; dims[1] = P.BN ? op.Cout / P.BN : 0; dims[2] = P.splits; dims[3] = P.BN;
     return 0;
 }
+int tc_conv_reduction(const Op& op) {
+    const TcParams& P = op.tc->P;
+    return P.splits <= 1 ? 0 : P.cluster_red ? 1 : 2;
+}
 
 }  // namespace b200trk

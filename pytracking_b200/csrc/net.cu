@@ -226,7 +226,9 @@ extern "C" int b200trk_net_dims(const b200trk_net_t* net, int dims[9]) {
     return 0;
 }
 
-namespace b200trk { int tc_conv_set_debug(Op& op, unsigned long long* buf); int tc_conv_grid(const Op& op, int dims[4]); }
+namespace b200trk {
+int tc_conv_set_debug(Op& op, unsigned long long* buf); int tc_conv_grid(const Op& op, int dims[4]); int tc_conv_reduction(const Op& op);
+}
 
 // Debug: attach (or detach, buf = NULL) a device buffer of [ctas][8] u64 phase time stamps to plan step `index`.
 extern "C" int b200trk_net_op_set_timing_buffer(b200trk_net_t* net, int index, unsigned long long* buf) {
@@ -241,6 +243,13 @@ extern "C" int b200trk_net_op_set_timing_buffer(b200trk_net_t* net, int index, u
 extern "C" int b200trk_net_op_grid(const b200trk_net_t* net, int index, int dims[4]) {
     B200_REQUIRE(net && dims && index >= 0 && index < (int)net->ops.size() && net->ops[index].tc, "net_op_grid: bad argument");
     return tc_conv_grid(net->ops[index], dims);
+}
+// Debug: how a tensor-core step as last configured reduces its split-K partials: 0 no split-K, 1 thread-block cluster (distributed
+// shared memory), 2 L2 workspace + arrival counters (more than 8 splits, or a cluster grid the device cannot hold at once).
+extern "C" int b200trk_net_op_splitk_reduction(const b200trk_net_t* net, int index, int* mode) {
+    B200_REQUIRE(net && mode && index >= 0 && index < (int)net->ops.size() && net->ops[index].tc, "net_op_splitk_reduction: bad argument");
+    *mode = tc_conv_reduction(net->ops[index]);
+    return 0;
 }
 
 extern "C" int b200trk_net_num_ops(const b200trk_net_t* net) { return net ? (int)net->ops.size() : 0; }

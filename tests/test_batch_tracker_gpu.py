@@ -79,10 +79,11 @@ def test_capacity_one_equals_solo_tracker_bitwise(kind):
     bt.close()
 
 
-def _mates_run(layout, n_frames, release_at, replacement):
+def _mates_run(layout, n_frames, release_at, replacement, cfg=BENCH, newton=None):
     """layout: {slot: (sequence, first step)}; at step release_at the slot of the mate `replacement[0]` gets sequence replacement[1].
-    Returns per slot the list of (box, score bits, filter bits) of every frame of its first sequence."""
-    bt = _batch(4)
+    Returns per slot the list of (box, score bits, filter bits) of every frame of its first sequence (capacity 4, configuration
+    cfg / newton as for _batch)."""
+    bt = _batch(4, cfg, newton)
     seqs = {slot: _seq(q, n_frames) for slot, (q, _) in layout.items()}
     pos = {slot: 0 for slot in layout}
     rec = {slot: [] for slot in layout}
@@ -111,10 +112,10 @@ def _mates_run(layout, n_frames, release_at, replacement):
     return rec
 
 
-def test_batch_mates_do_not_change_a_sequence():
+def check_batch_mates_do_not_change_a_sequence(cfg=BENCH, newton=None):
     n = 40
-    a = _mates_run({0: (0, 0), 1: (1, 0), 2: (2, 0), 3: (3, 0)}, n, release_at=20, replacement=(2, 7))
-    b = _mates_run({3: (0, 2), 0: (4, 0), 1: (5, 0), 2: (6, 0)}, n, release_at=25, replacement=(1, 8))
+    a = _mates_run({0: (0, 0), 1: (1, 0), 2: (2, 0), 3: (3, 0)}, n, release_at=20, replacement=(2, 7), cfg=cfg, newton=newton)
+    b = _mates_run({3: (0, 2), 0: (4, 0), 1: (5, 0), 2: (6, 0)}, n, release_at=25, replacement=(1, 8), cfg=cfg, newton=newton)
     qa, qb = a[0], b[3]
     assert len(qa) == len(qb) == n + 1
     for t in range(1, n + 1):                                  # frame 0 is the init step (its scores belong to no filter of the sequence)
@@ -122,6 +123,10 @@ def test_batch_mates_do_not_change_a_sequence():
         assert np.array_equal(qa[t][1], qb[t][1]), t
         assert np.array_equal(qa[t][2], qb[t][2]), t
     assert np.array_equal(qa[0][2], qb[0][2])
+
+
+def test_batch_mates_do_not_change_a_sequence():
+    check_batch_mates_do_not_change_a_sequence()
 
 
 def test_run_to_run_determinism():
@@ -157,10 +162,10 @@ def test_scores_match_solo_with_synchronised_filters():
     print("worst relative score difference batch(4) vs solo: %.3g" % worst)
 
 
-def _closed_loop(cfg, n):
+def _closed_loop(cfg, n, newton=None):
     from pytracking_b200 import shard, synth
     seqs = [_seq(q, n) for q in range(4)]
-    bt = _batch(4, cfg)
+    bt = _batch(4, cfg, newton)
     boxes_b = {s: [] for s in range(4)}
     bt.step({s: (seqs[s][0][0], {"init_bbox": seqs[s][1]}) for s in range(4)})
     for t in range(1, n + 1):
@@ -170,7 +175,7 @@ def _closed_loop(cfg, n):
     bt.close()
     boxes_s = {}
     for s in range(4):
-        trk = _solo(cfg)
+        trk = _solo(cfg, newton)
         trk.initialize(seqs[s][0][0], {"init_bbox": seqs[s][1]})
         boxes_s[s] = [trk.track(f)["target_bbox"] for f in seqs[s][0][1:]]
         trk.close()
@@ -181,11 +186,18 @@ def _closed_loop(cfg, n):
     return boxes_b, boxes_s, iou
 
 
-def test_closed_loop_stock_schedule_within_half_a_pixel_of_solo():
-    boxes_b, boxes_s, _ = _closed_loop(STOCK, 100)
+def check_closed_loop_within_half_a_pixel_of_solo(cfg=STOCK, newton=None):
+    boxes_b, boxes_s, _ = _closed_loop(cfg, 100, newton)
+    worst = 0.0
     for s in range(4):
         d = np.abs(np.array(boxes_b[s]) - np.array(boxes_s[s])).max()
+        worst = max(worst, float(d))
         assert d <= 0.5, (s, d)
+    return worst
+
+
+def test_closed_loop_stock_schedule_within_half_a_pixel_of_solo():
+    check_closed_loop_within_half_a_pixel_of_solo()
 
 
 def test_bench_schedule_iou_matches_solo():

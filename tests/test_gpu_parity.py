@@ -145,10 +145,16 @@ def test_backbone_golden(G, arch, size, seed, precision):
     assert _rel(l2, g[tag + "layer2"]) < 1e-4
     assert _rel(out["layer3"], g[tag + "layer3"]) < 1e-4
     assert _rel(out["classification"], g[tag + "clf"]) < 1e-4
-    # batch of 2 identical crops gives identical rows
-    out2 = eng.forward(torch.cat([im, im]))
-    assert torch.equal(out2["classification"][0], out2["classification"][1])
+    # a batch of two different crops: row 0 is the golden crop, row 1 another crop's batch-1 pass (a kernel that read one sample for
+    # every row, or mixed rows, fails one of the two)
+    im1 = synth.make_crop(seed + 1, 1, size).cuda()
+    one = eng.forward(im1)
+    out2 = eng.forward(torch.cat([im, im1]))
+    assert _rel(out2["layer2"][0] if size == 96 else out2["layer2"][0:1, ::8], g[tag + "layer2"]) < 1e-4
+    assert _rel(out2["layer3"][0], g[tag + "layer3"][0]) < 1e-4
     assert _rel(out2["classification"][0], g[tag + "clf"][0]) < 1e-4
+    for name in ("layer2", "layer3", "classification"):
+        assert _rel(out2[name][1], one[name][0]) < 1e-4, name
     eng.close()
 
 
