@@ -152,8 +152,8 @@ def dimp_label_maps(bb, params, out_sz, filter_size=4, feat_stride=16, bin_displ
     """optimizer.py:111-119: label y, target mask m = sigmoid(.), spatial weight v per sample; [n,Ho,Wo] each."""
     off = (filter_size % 2) / 2.0
     center = ((bb[:, :2] + bb[:, 2:] / 2) / feat_stride).flip((1,)) - off   # (row, col)
-    k0 = torch.arange(out_sz[0], dtype=bb.dtype).view(1, -1, 1)
-    k1 = torch.arange(out_sz[1], dtype=bb.dtype).view(1, 1, -1)
+    k0 = torch.arange(out_sz[0], dtype=bb.dtype, device=bb.device).view(1, -1, 1)
+    k1 = torch.arange(out_sz[1], dtype=bb.dtype, device=bb.device).view(1, 1, -1)
     d0 = k0 - center[:, 0].view(-1, 1, 1)
     d1 = k1 - center[:, 1].view(-1, 1, 1)
     rho = torch.sqrt(d0 * d0 + d1 * d1) / bin_displacement
@@ -211,12 +211,12 @@ def dimp_l2_sd_gn(w, feat, bb, sample_weight, log_step_length, filter_reg, num_i
     reg = max(float(filter_reg) ** 2, min_filter_reg ** 2)
     off = (k % 2) / 2.0
     center = ((bb[:, :2] + bb[:, 2:] / 2) / feat_stride).flip((1,)) - off
-    k0 = torch.arange(out_sz[0], dtype=torch.float32).view(1, -1, 1)
-    k1 = torch.arange(out_sz[1], dtype=torch.float32).view(1, 1, -1)
+    k0 = torch.arange(out_sz[0], dtype=bb.dtype, device=bb.device).view(1, -1, 1)
+    k1 = torch.arange(out_sz[1], dtype=bb.dtype, device=bb.device).view(1, 1, -1)
     g0 = torch.exp(-1.0 / (2 * gauss_sigma ** 2) * (k0 - center[:, 0].view(-1, 1, 1)) ** 2)
     g1 = torch.exp(-1.0 / (2 * gauss_sigma ** 2) * (k1 - center[:, 1].view(-1, 1, 1)) ** 2)
     y = g0 * g1
-    m = (y > hinge_threshold).float()
+    m = (y > hinge_threshold).to(y.dtype)
     y = y * m
     sw = math.sqrt(1.0 / n) if sample_weight is None else sample_weight.sqrt().reshape(n, 1, 1)
     iterates, losses = [w], []
@@ -248,7 +248,7 @@ def gn_sd_hinge(w, feat, train_label, sample_weight, filter_reg, num_iter, hinge
     n = feat.shape[0]
     k = w.shape[-1]
     sw = math.sqrt(1.0 / n) if sample_weight is None else sample_weight.sqrt().reshape(n, 1, 1)
-    m = ((train_label > hinge_threshold).float() + activation_leak).clamp(max=1.0)
+    m = ((train_label > hinge_threshold).to(train_label.dtype) + activation_leak).clamp(max=1.0)
     y = m * train_label
 
     def act_fn(s):
@@ -286,12 +286,12 @@ def prdimp_label_density(bb, out_sz, gauss_sigma, filter_size=4, feat_stride=16,
     """get_label_density (optimizer.py:331-353), gauss_sigma > 0."""
     off = (filter_size % 2) / 2.0
     center = ((bb[:, :2] + bb[:, 2:] / 2) / feat_stride).flip((1,)) - off
-    k0 = torch.arange(out_sz[0], dtype=torch.float32).view(1, -1, 1)
-    k1 = torch.arange(out_sz[1], dtype=torch.float32).view(1, 1, -1)
+    k0 = torch.arange(out_sz[0], dtype=bb.dtype, device=bb.device).view(1, -1, 1)
+    k1 = torch.arange(out_sz[1], dtype=bb.dtype, device=bb.device).view(1, 1, -1)
     g0 = torch.exp(-1.0 / (2 * gauss_sigma ** 2) * (k0 - center[:, 0].view(-1, 1, 1)) ** 2)
     g1 = torch.exp(-1.0 / (2 * gauss_sigma ** 2) * (k1 - center[:, 1].view(-1, 1, 1)) ** 2)
     gauss = (g0 / (2 * math.pi * gauss_sigma ** 2)) * g1
-    gauss = gauss * (gauss > label_threshold).float()
+    gauss = gauss * (gauss > label_threshold).to(gauss.dtype)
     if normalize_label:
         gauss = gauss / (gauss.sum(dim=(-2, -1), keepdim=True) + 1e-8)
     return (1.0 - label_shrink) * ((1.0 - uni_weight) * gauss + uni_weight / (out_sz[0] * out_sz[1]))
@@ -303,7 +303,7 @@ def softmax_reg(s, reg):
     flat = s.reshape(n, -1)
     if reg is None:
         return torch.softmax(flat, dim=1).reshape(s.shape)
-    ext = torch.cat((flat, torch.full((n, 1), float(reg))), dim=1)
+    ext = torch.cat((flat, torch.full((n, 1), float(reg), dtype=s.dtype, device=s.device)), dim=1)
     return torch.softmax(ext, dim=1)[:, :-1].reshape(s.shape)
 
 
@@ -320,7 +320,7 @@ def prdimp_sd_newton(w, feat, bb, sample_weight, log_step_length, filter_reg, nu
     p = prdimp_label_density(bb, out_sz, gauss_sigma, k, feat_stride, label_threshold, normalize_label,
                              label_shrink, uni_weight)
     if sample_weight is None:
-        sw = torch.full((n, 1, 1), 1.0 / n)
+        sw = torch.full((n, 1, 1), 1.0 / n, dtype=feat.dtype, device=feat.device)
     else:
         sw = sample_weight.reshape(n, 1, 1)
     exp_reg = 0.0 if softmax_reg_val is None else math.exp(softmax_reg_val)

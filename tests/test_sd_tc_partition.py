@@ -1,4 +1,4 @@
-"""Invariants of the unit decomposition of the tcgen05 steepest-descent kernel (pytracking_b200/csrc/sd_tc.cu).
+"""Invariants of the unit decomposition of the tensor-core (wgmma) steepest-descent kernel (pytracking_b200/csrc/sd_tc.cu).
 
 The kernel deals the 128 x 32 operand tiles ("units") of a sweep to the CTAs as contiguous ranges [lo(b), lo(b+1)) with
 lo(b) = floor(b U / G), and every consumer re-derives, with integer arithmetic only, which CTA produced which partial:
@@ -36,9 +36,9 @@ def test_owner_is_the_cta_whose_range_holds_the_unit(U, G):
         assert 0 <= b < G and lo(U, G, b) <= u < lo(U, G, b + 1)
 
 
+@pytest.mark.parametrize("G", [132, 114, 148], ids=["h100_sxm", "h100_pcie", "g148"])
 @pytest.mark.parametrize("n,C,fs", [(1, 512, 18), (3, 256, 18), (15, 512, 18), (50, 512, 18), (50, 128, 22), (15, 512, 22), (33, 384, 18)])
-def test_apply_segments_and_gradient_contributors(n, C, fs):
-    G = 148
+def test_apply_segments_and_gradient_contributors(n, C, fs, G):
     npx = fs * fs
     kbt, npt, kba, nchk = (npx + 31) // 32, (npx + 127) // 128, C // 32, C // 128
     UA, UT = n * npt * kba, nchk * n * kbt
