@@ -264,17 +264,35 @@ int b200trk_net_forward(b200trk_net_t* net, const float* crop, int S,
  * iou4 [S,C,h/16,w/16] (NULL skips the branch); b200trk_net_iou_dims: {C3,H3,W3, C4,H4,W4}. */
 int b200trk_net_attach_iou_head(b200trk_net_t* net, const b200trk_conv_desc_t* convs);
 int b200trk_net_iou_dims(const b200trk_net_t* net, int dims[6]);
+/* AtomIoUNet's reference branch (get_modulation, ltr/models/bbreg/atom_iou_net.py:150-162): convs = {conv3_1r, conv4_1r}, conv3x3 +
+ * bias + eval-mode BN + ReLU on layer2 / layer3. Plan steps (kind 3) that no forward pass runs, for b200trk_iou_modulation_get;
+ * visible to the net_op_* introspection calls; not counted in b200trk_net_flops. */
+int b200trk_net_attach_iou_ref(b200trk_net_t* net, const b200trk_conv_desc_t* convs);
 /* The IoU branch alone on the layer2 / layer3 activations the most recent forward pass (same S) left in the arena -- the reference
  * calls get_iou_feat lazily, only on frames that refine the box (dimp.py:657-658). */
 int b200trk_net_iou_from_arena(b200trk_net_t* net, int S, float* iou3, float* iou4, b200trk_stream_t stream);
 int b200trk_net_forward_iou(b200trk_net_t* net, const float* crop, int S, float* layer2, float* layer3, float* clf,
                             float* iou3, float* iou4, b200trk_stream_t stream);
+/* FilterInitializerLinear (ltr/models/target_classifier/initializer.py:118-173), the learnt first-frame filter of DiMP-50 / PrDiMP-50.
+ * Attach: conv = classifier.filter_initializer.filter_conv (Cc -> Cc, odd k, padding k // 2, bias), filter_size = the classifier's k,
+ * filter_norm / pool_square = the constructor arguments of the same names (both False in dimpnet50 and klcedimpnet50). The convolution
+ * becomes a plan step (kind 3, after an NCHW -> NHWC import step of kind 6) that no forward pass runs; it is visible to the net_op_*
+ * introspection calls. Attaching does not change b200trk_net_flops.
+ * Run: clf [S,Cc,Hc,Wc] normalised classification features (device, as b200trk_net_forward writes them), S <= max_batch; boxes [n,4]
+ * (x, y, w, h) in crop pixels, box r on image images[r] (images NULL: box r on image r), 1 <= n <= 16; writes filter [1,Cc,k,k] =
+ * the mean over the n pooled boxes (the initialiser's filter of n images). Bitwise deterministic.
+ * A tracker state of this network starts its optimiser from this filter; its filter_size must equal the one attached here
+ * (initialize refuses a mismatch). */
+int b200trk_net_attach_filter_init(b200trk_net_t* net, const b200trk_conv_desc_t* conv, int filter_size, int filter_norm, int pool_square);
+int b200trk_net_filter_init_attached(const b200trk_net_t* net);
+int b200trk_net_filter_init(b200trk_net_t* net, const float* clf, int S, int n, const int* images, const float* boxes, float* filter,
+                            b200trk_stream_t stream);
 /* Query output geometry: dims = {C2,H2,W2, C3,H3,W3, Cc,Hc,Wc}. */
 int b200trk_net_dims(const b200trk_net_t* net, int dims[9]);
 /* FLOPs (2*MAC) of one forward pass at batch 1, for roofline accounting. */
 double b200trk_net_flops(const b200trk_net_t* net);
 /* Introspection of the execution plan (tests / profiling): number of plan steps; per step
- * info = {kind (0 preprocess,1 stem,2 maxpool,3 conv,4 export,5 l2norm), Cin, Cout, k, stride, Hout, Wout, runs_on_tensor_cores};
+ * info = {kind (0 preprocess,1 stem,2 maxpool,3 conv,4 export,5 l2norm,6 nchw import), Cin, Cout, k, stride, Hout, Wout, runs_on_tensor_cores};
  * and a device-to-device copy of a step's NHWC output activation [S,Hout,Wout,Cout] after a forward pass. */
 int b200trk_net_num_ops(const b200trk_net_t* net);
 int b200trk_net_op_info(const b200trk_net_t* net, int index, int info[8]);
@@ -427,6 +445,22 @@ typedef struct {
     const float* weight; const float* bias; const float* bn_gamma; const float* bn_beta; const float* bn_mean; const float* bn_var;
 } b200trk_linear_block_t;
 typedef struct b200trk_iou_predictor b200trk_iou_predictor_t;
+typedef struct b200trk_iou_modulation b200trk_iou_modulation_t;
+
+/* AtomIoUNet.get_modulation (ltr/models/bbreg/atom_iou_net.py:138-170) after conv3_1r / conv4_1r: fc3_1r (conv3x3 valid on the 3x3
+ * PrRoIPool at 1/8 of c3_r: weight [D, C3, 3, 3] read as [D, 9 C3]), concatenation with the 1x1 PrRoIPool at 1/16 of c4_r, fc34_3r /
+ * fc34_4r (conv1x1: weight [M, D + C4]); each block conv bias + eval-mode BN (eps 1e-5, folded in double) + ReLU. HOST pointers.
+ * DiMP-50 / PrDiMP-50: C3 = 128, C4 = 256, D = M3 = M4 = 256. */
+int b200trk_iou_modulation_create(b200trk_iou_modulation_t** out, const b200trk_linear_block_t* fc3_1r, const b200trk_linear_block_t* fc34_3r,
+                                  const b200trk_linear_block_t* fc34_4r, int C3, int C4, int D, int M3, int M4);
+int b200trk_iou_modulation_destroy(b200trk_iou_modulation_t* m);
+/* dims = {M3, M4} */
+int b200trk_iou_modulation_dims(const b200trk_iou_modulation_t* m, int dims[2]);
+/* The modulation vectors of R boxes (1..16) on the layer2 / layer3 activations the most recent forward pass of batch S left in the
+ * arena of `net` (b200trk_net_attach_iou_ref attached): box r (x, y, w, h, crop pixels) on image images[r] (NULL: image r) ->
+ * mod3 [R,M3], mod4 [R,M4] (device). Fixed-order sums: bitwise deterministic, and each box's vectors depend on its image and box only. */
+int b200trk_iou_modulation_get(b200trk_iou_modulation_t* m, b200trk_net_t* net, int S, int R, const int* images, const float* boxes,
+                               float* mod3, float* mod4, b200trk_stream_t stream);
 
 /* The prediction head of AtomIoUNet (ltr/models/bbreg/atom_iou_net.py:39-48): fc3_rt = LinearBlock(C3*P3*P3 -> D3) on the P3 x P3
  * PrRoIPool (scale 1/8) of the layer2 IoU features, fc4_rt = LinearBlock(C4*P4*P4 -> D4) on the P4 x P4 pool (scale 1/16) of the layer3
@@ -565,9 +599,16 @@ int b200trk_dimp_tracker_adopt(b200trk_dimp_tracker_t* t, int H, int W, const fl
 /* IoUNet refinement (DiMP.refine_target_box, dimp.py:650-723) for this tracker: `pred` = the prediction head, modulation3 / modulation4 =
  * HOST [C3] / [C4] modulation vectors (DiMP.init_iou_net, dimp.py:509-540: get_modulation of the first-frame target, computed by the
  * caller -- e.g. the reference's own initialisation above the plug-in). The network of the tracker's state must have the IoU feature
- * branch attached (b200trk_net_attach_iou_head). */
+ * branch attached (b200trk_net_attach_iou_head). NULL modulation3 and modulation4: computed natively by initialize (see below). */
 int b200trk_dimp_tracker_attach_iounet(b200trk_dimp_tracker_t* t, b200trk_iou_predictor_t* pred, const float* modulation3,
                                        const float* modulation4);
+/* Native first-frame modulation: attach the modulation head (the tracker's network needs b200trk_net_attach_iou_ref) before the
+ * first initialize, then call b200trk_dimp_tracker_attach_iounet with modulation3 = modulation4 = NULL. initialize then computes the
+ * vectors from its init pass -- the identity sample at init_target_box, as DiMP.init_iou_net does without iounet_augmentation
+ * (dimp.py:509-540; the mean over one box is that box's vectors). Both attachments are refused after initialize. */
+int b200trk_dimp_tracker_attach_modulation_head(b200trk_dimp_tracker_t* t, b200trk_iou_modulation_t* head);
+/* Host copies of the modulation vectors the IoUNet uses (C3 and C4 floats of b200trk_net_iou_dims). */
+int b200trk_dimp_tracker_modulation(const b200trk_dimp_tracker_t* t, float* modulation3, float* modulation4);
 /* The uniform [0,1) numbers of the next frame's random proposals (`torch.rand(num_init_random_boxes, 4)`, dimp.py:667), HOST
  * [num_init_random_boxes * 4]; consumed by the next track call. Without it the tracker draws from its own generator. */
 int b200trk_dimp_tracker_set_proposal_noise(b200trk_dimp_tracker_t* t, const float* u01, int count);

@@ -122,6 +122,16 @@ SIGNATURES = {
     "b200trk_net_attach_iou_head": (_I, [_VP, C.POINTER(ConvDesc)]),
     "b200trk_net_iou_from_arena": (_I, [_VP, _I, _VP, _VP, _VP]),
     "b200trk_net_iou_dims": (_I, [_VP, C.POINTER(C.c_int * 6)]),
+    "b200trk_net_attach_iou_ref": (_I, [_VP, C.POINTER(ConvDesc)]),
+    "b200trk_iou_modulation_create": (_I, [C.POINTER(_VP), C.POINTER(LinearBlock), C.POINTER(LinearBlock), C.POINTER(LinearBlock), _I, _I, _I, _I, _I]),
+    "b200trk_iou_modulation_destroy": (_I, [_VP]),
+    "b200trk_iou_modulation_dims": (_I, [_VP, C.POINTER(C.c_int * 2)]),
+    "b200trk_iou_modulation_get": (_I, [_VP, _VP, _I, _I, _VP, _VP, _VP, _VP, _VP]),
+    "b200trk_dimp_tracker_attach_modulation_head": (_I, [_VP, _VP]),
+    "b200trk_dimp_tracker_modulation": (_I, [_VP, _VP, _VP]),
+    "b200trk_net_attach_filter_init": (_I, [_VP, C.POINTER(ConvDesc), _I, _I, _I]),
+    "b200trk_net_filter_init_attached": (_I, [_VP]),
+    "b200trk_net_filter_init": (_I, [_VP, _VP, _I, _I, _VP, _VP, _VP, _VP]),
     "b200trk_net_forward_iou": (_I, [_VP, _VP, _I, _VP, _VP, _VP, _VP, _VP, _VP]),
     "b200trk_net_dims": (_I, [_VP, C.POINTER(C.c_int * 9)]),
     "b200trk_net_flops": (C.c_double, [_VP]),

@@ -13,15 +13,17 @@ import torch
 
 from . import _lib
 from .engine import BackboneEngine
-from .frame_engine import _view, optimizer_args
+from .frame_engine import _view, attach_filter_init, optimizer_args
 from .tracker import frame_pointer, tracker_settings
 
 
 class DiMPBatchTracker:
     """`state_dict`, `params`, `arch`, `newton` as for `DiMPTracker` (newton=None: DiMP's GN optimiser; a dict: PrDiMP's Newton
-    optimiser, whose softmax_reg the localisation then uses).  use_iou_net must be False."""
+    optimiser, whose softmax_reg the localisation then uses), `filter_init`, `init_filter_norm`, `init_pool_square` as for
+    `DiMPTracker`.  use_iou_net must be False."""
 
-    def __init__(self, state_dict, params, capacity, arch="resnet50", newton=None, device=None, precision=0, **param_overrides):
+    def __init__(self, state_dict, params, capacity, arch="resnet50", newton=None, device=None, precision=0, filter_init="zero",
+                 init_filter_norm=False, init_pool_square=False, **param_overrides):
         self.params, newton = tracker_settings(params, newton, **param_overrides)
         p = self.params
         if p.use_iou_net:
@@ -30,6 +32,7 @@ class DiMPBatchTracker:
             raise RuntimeError("DiMPBatchTracker: capacity=%r outside 1..16" % (capacity,))
         self.capacity = int(capacity)
         self.backbone = BackboneEngine(state_dict, arch, 4, self.capacity, p.image_sample_size, precision, device)
+        attach_filter_init(self.backbone, state_dict, filter_init, 4, init_filter_norm, init_pool_square)
         self.device = self.backbone.device
         args, _, _ = optimizer_args(state_dict, newton)
         create = "dimp_batch_create" if newton is None else "prdimp_batch_create"

@@ -86,6 +86,8 @@ struct b200trk_dimp_tracker {
     b200trk_iou_predictor_t* iou_pred = nullptr;
     float *mod3 = nullptr, *mod4 = nullptr, *iou3 = nullptr, *iou4 = nullptr, *boxes_dev = nullptr;   // device
     float* boxes_host = nullptr;                     // pinned: [16][4] boxes + [16] IoUs
+    b200trk_iou_modulation_t* mod_head = nullptr;    // get_modulation; with mod_native, initialize computes mod3 / mod4
+    int mod_native = 0;
     int iou_dims[6] = {0, 0, 0, 0, 0, 0};
     float pos_iounet[2] = {0, 0}; int has_pos_iounet = 0;
     std::vector<float> noise;                        // uniform numbers for the next frame's random proposals
@@ -526,23 +528,57 @@ extern "C" int b200trk_dimp_tracker_set_proposal_noise(b200trk_dimp_tracker_t* t
     return 0;
 }
 
+extern "C" int b200trk_dimp_tracker_attach_modulation_head(b200trk_dimp_tracker_t* t, b200trk_iou_modulation_t* head) {
+    B200_REQUIRE(t && head, "dimp_tracker_attach_modulation_head: null pointer");
+    B200_REQUIRE(t->st, "dimp_tracker_attach_modulation_head: host-logic-only tracker");
+    B200_REQUIRE(!t->initialized, "dimp_tracker_attach_modulation_head: refused after initialize (the modulation comes from the first frame)");
+    B200_REQUIRE(!t->mod_head, "dimp_tracker_attach_modulation_head: already attached");
+    B200_REQUIRE(t->st->net->iouref.op[0] >= 0, "dimp_tracker_attach_modulation_head: the network has no conv3_1r / conv4_1r "
+                 "(b200trk_net_attach_iou_ref)");
+    t->mod_head = head;
+    return 0;
+}
+
 extern "C" int b200trk_dimp_tracker_attach_iounet(b200trk_dimp_tracker_t* t, b200trk_iou_predictor_t* pred, const float* modulation3,
                                                   const float* modulation4) {
-    B200_REQUIRE(t && pred && modulation3 && modulation4, "dimp_tracker_attach_iounet: null pointer");
+    B200_REQUIRE(t && pred, "dimp_tracker_attach_iounet: null pointer");
+    B200_REQUIRE((modulation3 == nullptr) == (modulation4 == nullptr), "dimp_tracker_attach_iounet: give both modulation vectors or neither");
+    const bool native = modulation3 == nullptr;
     B200_REQUIRE(t->st, "dimp_tracker_attach_iounet: host-logic-only tracker");
     B200_REQUIRE(!t->iou_pred, "dimp_tracker_attach_iounet: already attached");
+    B200_REQUIRE(!native || t->mod_head, "dimp_tracker_attach_iounet: no modulation vectors and no modulation head "
+                 "(b200trk_dimp_tracker_attach_modulation_head)");
+    B200_REQUIRE(!native || !t->initialized, "dimp_tracker_attach_iounet: native modulation is computed by initialize; attach before it");
     if (int e = b200trk_net_iou_dims(t->st->net, t->iou_dims)) return e;
     B200_REQUIRE(t->iou_dims[0] > 0, "dimp_tracker_attach_iounet: the network has no IoU feature branch (b200trk_net_attach_iou_head)");
     const int C3 = t->iou_dims[0], C4 = t->iou_dims[3];
+    if (native) {
+        int md[2];
+        if (int e = b200trk_iou_modulation_dims(t->mod_head, md)) return e;
+        B200_REQUIRE(md[0] == C3 && md[1] == C4, "dimp_tracker_attach_iounet: the modulation head gives %d / %d values, the IoU features have "
+                     "%d / %d channels", md[0], md[1], C3, C4);
+    }
     B200_CHECK_CUDA(cudaMalloc((void**)&t->mod3, C3 * sizeof(float)));
     B200_CHECK_CUDA(cudaMalloc((void**)&t->mod4, C4 * sizeof(float)));
-    B200_CHECK_CUDA(cudaMemcpy(t->mod3, modulation3, C3 * sizeof(float), cudaMemcpyHostToDevice));
-    B200_CHECK_CUDA(cudaMemcpy(t->mod4, modulation4, C4 * sizeof(float), cudaMemcpyHostToDevice));
+    if (!native) {
+        B200_CHECK_CUDA(cudaMemcpy(t->mod3, modulation3, C3 * sizeof(float), cudaMemcpyHostToDevice));
+        B200_CHECK_CUDA(cudaMemcpy(t->mod4, modulation4, C4 * sizeof(float), cudaMemcpyHostToDevice));
+    }
     B200_CHECK_CUDA(cudaMalloc((void**)&t->iou3, (size_t)C3 * t->iou_dims[1] * t->iou_dims[2] * sizeof(float)));
     B200_CHECK_CUDA(cudaMalloc((void**)&t->iou4, (size_t)C4 * t->iou_dims[4] * t->iou_dims[5] * sizeof(float)));
     B200_CHECK_CUDA(cudaMalloc((void**)&t->boxes_dev, 16 * 5 * sizeof(float)));
     B200_CHECK_CUDA(cudaMallocHost((void**)&t->boxes_host, 16 * 5 * sizeof(float)));
     t->iou_pred = pred;
+    t->mod_native = native ? 1 : 0;
+    return 0;
+}
+
+extern "C" int b200trk_dimp_tracker_modulation(const b200trk_dimp_tracker_t* t, float* modulation3, float* modulation4) {
+    B200_REQUIRE(t && modulation3 && modulation4, "dimp_tracker_modulation: null pointer");
+    B200_REQUIRE(t->iou_pred, "dimp_tracker_modulation: no IoUNet attached");
+    B200_CHECK_CUDA(cudaDeviceSynchronize());
+    B200_CHECK_CUDA(cudaMemcpy(modulation3, t->mod3, t->iou_dims[0] * sizeof(float), cudaMemcpyDeviceToHost));
+    B200_CHECK_CUDA(cudaMemcpy(modulation4, t->mod4, t->iou_dims[3] * sizeof(float), cudaMemcpyDeviceToHost));
     return 0;
 }
 
@@ -583,11 +619,24 @@ extern "C" int b200trk_dimp_localize(const float* scores, int S, int Ho, int Wo,
     return 0;
 }
 
-// The device half of initialize (dimp.py:601-602, FilterInitializerZero): the first frame's features `feat` become sample 0 with box
-// `box`, and num_iter iterations run from the zero filter.  The reference passes sample_weight = None, which both optimisers read as
-// 1/num_images (optimizer.py:122-123 GN, :387-388 Newton): with one sample that is the weight 1 uploaded here.
-static int first_frame_update(b200trk_dimp_state* s, const float* feat, const float box[4], int num_iter, cudaStream_t st) {
-    B200_CHECK_CUDA(cudaMemsetAsync(s->filter, 0, (size_t)s->Cc * s->ksz * s->ksz * sizeof(float), st));
+// The device half of initialize (dimp.py:601-602): the first frame's features `feat` become sample 0 with box `box`, and num_iter
+// iterations run from the initial filter.  That is FilterInitializerLinear's when the network has one attached -- the caller has run its
+// filter_conv on the S feature maps of the arena, of which this sequence's is `image` -- else FilterInitializerZero's zero filter.  The
+// reference passes sample_weight = None, which both optimisers read as 1/num_images (optimizer.py:122-123 GN, :387-388 Newton): with one
+// sample that is the weight 1 uploaded here.
+// A learnt initialiser attached to the state's network must make filters of the state's size
+static int filter_init_ok(const b200trk_dimp_state* s, const char* what) {
+    B200_REQUIRE(s->net->finit.conv_op < 0 || s->net->finit.ksz == s->ksz, "%s: the network's filter initialiser makes %dx%d filters, the "
+                 "tracker's state holds %dx%d", what, s->net->finit.ksz, s->net->finit.ksz, s->ksz, s->ksz);
+    return 0;
+}
+
+static int first_frame_update(b200trk_dimp_state* s, const float* feat, int S, int image, const float box[4], int num_iter, cudaStream_t st) {
+    if (s->net->finit.conv_op >= 0) {
+        if (int e = filter_init_pool(s->net, S, 1, &image, box, s->filter, st)) return e;
+    } else {
+        B200_CHECK_CUDA(cudaMemsetAsync(s->filter, 0, (size_t)s->Cc * s->ksz * s->ksz * sizeof(float), st));
+    }
     B200_CHECK_CUDA(cudaMemsetAsync(s->sw, 0, (size_t)s->memory_size * sizeof(float), st));
     const float one = 1.f;
     return dimp_state_insert(s, feat, 0, box, &one, 1, num_iter, st);
@@ -605,6 +654,7 @@ extern "C" int b200trk_dimp_tracker_initialize_host(b200trk_dimp_tracker_t* t, c
                                                     b200trk_stream_t stream) {
     B200_REQUIRE(t && image && init_bbox, "dimp_tracker_initialize_host: null pointer");
     B200_REQUIRE(t->st, "dimp_tracker_initialize_host: host-logic-only tracker (created without a device state)");
+    if (int e = filter_init_ok(t->st, "dimp_tracker_initialize_host")) return e;
     cudaStream_t st = (cudaStream_t)stream;
     b200trk_dimp_state* s = t->st;
     b200trk_crop_geom_t g; float box[4];
@@ -613,7 +663,13 @@ extern "C" int b200trk_dimp_tracker_initialize_host(b200trk_dimp_tracker_t* t, c
     const int iss = t->p.image_sample_size;
     if (int e = b200trk_sample_patch(image, H, W, &g, iss, iss, s->crop, stream)) return e;
     if (int e = b200trk_net_forward(s->net, s->crop, 1, nullptr, nullptr, s->clf, stream)) return e;
-    if (int e = first_frame_update(s, s->clf, box, t->p.net_opt_iter > 0 ? t->p.net_opt_iter : 0, st)) return e;
+    if (s->net->finit.conv_op >= 0)
+        if (int e = filter_init_conv(s->net, s->clf, 1, st)) return e;
+    if (int e = first_frame_update(s, s->clf, 1, 0, box, t->p.net_opt_iter > 0 ? t->p.net_opt_iter : 0, st)) return e;
+    // DiMP.init_iou_net (dimp.py:509-540) without iounet_augmentation: get_modulation of the identity sample at init_target_box, on the
+    // layer2 / layer3 activations of this init pass; the mean over that one box is its own vectors
+    if (t->mod_native)
+        if (int e = b200trk_iou_modulation_get(t->mod_head, s->net, 1, 1, nullptr, box, t->mod3, t->mod4, stream)) return e;
     B200_CHECK_CUDA(cudaStreamSynchronize(st));
     return 0;
 }
@@ -814,6 +870,7 @@ static int batch_step(b200trk_dimp_batch* b, const b200trk_batch_item_t* items, 
         std::snprintf(what[k], sizeof(what[k]), "dimp_batch_step: slot %d", it.slot);
         B200_REQUIRE(it.image && it.H > 0 && it.W > 0, "%s: no frame or an empty one (%dx%d)", what[k], it.H, it.W);
         if (it.init) {
+            if (int e = filter_init_ok(b->t[it.slot]->st, what[k])) return e;
             B200_REQUIRE(it.init_bbox[2] > 0 && it.init_bbox[3] > 0, "%s: init box of size %gx%g", what[k], it.init_bbox[2], it.init_bbox[3]);
         } else if (int e = tracking_ok(b->t[it.slot], it.H, it.W, what[k])) {
             return e;
@@ -884,7 +941,10 @@ static int batch_step(b200trk_dimp_batch* b, const b200trk_batch_item_t* items, 
         if (int e = b200trk_dimp_tracker_commit(t, &sa.g[k], &b->loc_host[j], &infos[k], nullptr)) return e;
         if (int e = frame_update(t, b->clf + plane * slot, &infos[k], st)) return e;
     }
-    // initialisation, as b200trk_dimp_tracker_initialize_host
+    // initialisation, as b200trk_dimp_tracker_initialize_host; a learnt initialiser's convolution runs once, at batch S like the forward
+    const bool any_init = std::any_of(items, items + n, [](const b200trk_batch_item_t& it) { return it.init != 0; });
+    if (any_init && b->net->finit.conv_op >= 0)
+        if (int e = filter_init_conv(b->net, b->clf, b->cap, st)) return e;
     for (int k = 0; k < n; ++k) {
         if (!items[k].init) continue;
         const int slot = items[k].slot;
@@ -893,7 +953,7 @@ static int batch_step(b200trk_dimp_batch* b, const b200trk_batch_item_t* items, 
         info->crop = sa.g[k];
         for (int i = 0; i < 4; ++i) { info->bbox[i] = f32(items[k].init_bbox[i]); info->target_box[i] = box[k][i]; }
         info->updated = 1; info->n_stored = 1; info->num_iter = b->p.net_opt_iter > 0 ? b->p.net_opt_iter : 0;
-        if (int e = first_frame_update(b->t[slot]->st, b->clf + plane * slot, box[k], info->num_iter, st)) return e;
+        if (int e = first_frame_update(b->t[slot]->st, b->clf + plane * slot, b->cap, slot, box[k], info->num_iter, st)) return e;
     }
     return 0;
 }

@@ -333,6 +333,107 @@ extern "C" int b200trk_net_attach_iou_head(b200trk_net_t* net, const b200trk_con
     return 0;
 }
 
+// One convolution step of the plan at batch S: the tensor-core kernel where the step has one, else the fp32 CUDA-core kernel.
+static int conv_step(b200trk_net_t* net, const Op& op, int S, cudaStream_t st) {
+    if (op.tc) return tc_conv_launch(net, op, S, st);
+    ConvShape sh{S, op.Hin, op.Win, op.Cin, op.Hout, op.Wout, op.Cout, op.k, op.stride, op.pad};
+    ConvEpilogue ep{op.bias, op.res >= 0 ? net->bufs[op.res] : nullptr, op.relu};
+    return launch_conv_fp32(net->bufs[op.in], op.w, net->bufs[op.out], sh, ep, net->splitk_ws, net->splitk_ws_floats, net->sms, st);
+}
+
+// FilterInitializerLinear.filter_conv (ltr/models/target_classifier/initializer.py:130,163) appended to the plan.  It reads the
+// normalised classification features, which a forward pass only writes NCHW to the caller's `clf` (InstanceL2Norm is fused into that
+// export): an import step copies them back into an NHWC arena buffer, so the convolution takes the plan's own paths and the forward pass
+// stays as it is.  The step's output is also kept NCHW for PrRoIPool.  The initialiser runs once per sequence, so its FLOPs are not
+// counted in b200trk_net_flops (one frame's forward pass).
+extern "C" int b200trk_net_attach_filter_init(b200trk_net_t* net, const b200trk_conv_desc_t* conv, int filter_size, int filter_norm,
+                                              int pool_square) {
+    B200_REQUIRE(net && conv, "net_attach_filter_init: null pointer");
+    B200_REQUIRE(net->finit.conv_op < 0, "net_attach_filter_init: already attached");
+    B200_REQUIRE(net->dims[6] > 0, "net_attach_filter_init: the network has no classification head");
+    B200_REQUIRE(filter_size >= 1 && filter_size <= 8, "net_attach_filter_init: filter_size=%d (1..8)", filter_size);
+    B200_REQUIRE(conv->k % 2 == 1, "net_attach_filter_init: filter_conv kernel size %d must be odd (padding k // 2)", conv->k);
+    const int C = net->dims[6], H = net->dims[7], W = net->dims[8];
+    // every refusal before the plan changes
+    B200_REQUIRE(conv->weight && conv->cin == C && conv->cout == C && conv->stride == 1 && conv->pad == conv->k / 2,
+                 "net_attach_filter_init: filter_conv is (cin=%d,cout=%d,k=%d,s=%d,p=%d), the head needs (%d,%d,k,1,k/2)", conv->cin,
+                 conv->cout, conv->k, conv->stride, conv->pad, C, C);
+    drop_graph(net);
+    const double flops = net->flops;
+    Op imp; imp.kind = OP_NCHW_IMPORT; imp.init = 1;
+    imp.Hin = imp.Hout = H; imp.Win = imp.Wout = W; imp.Cin = imp.Cout = C;
+    if (int e = new_buf(net, (size_t)H * W * C, &imp.out)) return e;
+    net->ops.push_back(imp);
+    Builder B{net, conv, 1};
+    int o, h, w;
+    if (int e = B.add_conv(imp.out, -1, H, W, C, C, conv->k, 1, conv->k / 2, 0, &o, &h, &w)) return e;
+    net->ops.back().init = 1;
+    auto& f = net->finit;
+    f.import_op = (int)net->ops.size() - 2; f.conv_op = (int)net->ops.size() - 1;
+    f.ksz = filter_size; f.norm = filter_norm != 0; f.square = pool_square != 0;
+    if (int e = new_buf(net, (size_t)H * W * C, &f.nchw)) return e;
+    if (int e = dev_alloc(net, &f.rois, 5 * 16)) return e;
+    if (int e = dev_alloc(net, &f.pooled, (size_t)16 * C * filter_size * filter_size)) return e;
+    net->flops = flops;
+    return 0;
+}
+
+// AtomIoUNet's reference branch of get_modulation (ltr/models/bbreg/atom_iou_net.py:30-35,150-162): convs = {conv3_1r, conv4_1r},
+// conv3x3 + bias + eval-mode BN + ReLU on the layer2 / layer3 activations in the arena.  Plan steps that no forward pass runs (the
+// reference evaluates them on the first frame only); their FLOPs are not counted in b200trk_net_flops.
+extern "C" int b200trk_net_attach_iou_ref(b200trk_net_t* net, const b200trk_conv_desc_t* convs) {
+    B200_REQUIRE(net && convs, "net_attach_iou_ref: null pointer");
+    B200_REQUIRE(net->iouref.op[0] < 0, "net_attach_iou_ref: already attached");
+    B200_REQUIRE(net->feat_buf[0] >= 0 && net->feat_buf[1] >= 0, "net_attach_iou_ref: the network has no layer2 / layer3 outputs");
+    for (int lvl = 0; lvl < 2; ++lvl) {
+        const b200trk_conv_desc_t& d = convs[lvl];
+        B200_REQUIRE(d.weight && d.cin == net->feat_hw[lvl][0] && d.k == 3 && d.stride == 1 && d.pad == 1 && d.cout > 0,
+                     "net_attach_iou_ref: conv%d_1r is (cin=%d,k=%d,s=%d,p=%d), layer%d needs (%d,3,1,1)", lvl + 3, d.cin, d.k, d.stride,
+                     d.pad, lvl + 2, net->feat_hw[lvl][0]);
+    }
+    drop_graph(net);
+    const double flops = net->flops;
+    auto& f = net->iouref;
+    for (int lvl = 0; lvl < 2; ++lvl) {
+        const int C = net->feat_hw[lvl][0], H = net->feat_hw[lvl][1], W = net->feat_hw[lvl][2];
+        Builder B{net, convs + lvl, 1};
+        int o, h, w;
+        if (int e = B.add_conv(net->feat_buf[lvl], -1, H, W, C, convs[lvl].cout, 3, 1, 1, 1, &o, &h, &w)) return e;
+        net->ops.back().init = 1;
+        f.op[lvl] = (int)net->ops.size() - 1;
+        if (int e = new_buf(net, (size_t)h * w * convs[lvl].cout, &f.nchw[lvl])) return e;
+        f.dims[3 * lvl] = convs[lvl].cout; f.dims[3 * lvl + 1] = h; f.dims[3 * lvl + 2] = w;
+    }
+    net->flops = flops;
+    return 0;
+}
+
+namespace b200trk {
+int iou_ref_conv(b200trk_net* net, int S, cudaStream_t st) {
+    const auto& f = net->iouref;
+    B200_REQUIRE(f.op[0] >= 0, "iou_modulation: the network has no conv3_1r / conv4_1r (b200trk_net_attach_iou_ref)");
+    B200_REQUIRE(S >= 1 && S <= net->max_batch, "iou_modulation: batch %d outside [1,%d]", S, net->max_batch);
+    for (int lvl = 0; lvl < 2; ++lvl) {
+        const Op& op = net->ops[f.op[lvl]];
+        if (int e = conv_step(net, op, S, st)) return e;
+        if (int e = launch_nhwc_to_nchw(net->bufs[op.out], net->bufs[f.nchw[lvl]], S, op.Hout * op.Wout, op.Cout, st)) return e;
+    }
+    return 0;
+}
+
+int filter_init_conv(b200trk_net* net, const float* clf, int S, cudaStream_t st) {
+    const auto& f = net->finit;
+    B200_REQUIRE(f.conv_op >= 0, "filter_init: no filter initialiser is attached (b200trk_net_attach_filter_init)");
+    B200_REQUIRE(clf, "filter_init: null pointer");
+    B200_REQUIRE(S >= 1 && S <= net->max_batch, "filter_init: batch %d outside [1,%d]", S, net->max_batch);
+    const Op& imp = net->ops[f.import_op];
+    const Op& conv = net->ops[f.conv_op];
+    if (int e = launch_nchw_to_nhwc(clf, net->bufs[imp.out], S, imp.Hout * imp.Wout, imp.Cout, st)) return e;
+    if (int e = conv_step(net, conv, S, st)) return e;
+    return launch_nhwc_to_nchw(net->bufs[conv.out], net->bufs[f.nchw], S, conv.Hout * conv.Wout, conv.Cout, st);
+}
+}  // namespace b200trk
+
 // The IoU branch alone, on the layer2 / layer3 activations the most recent forward pass of batch S left in the arena.
 extern "C" int b200trk_net_iou_from_arena(b200trk_net_t* net, int S, float* iou3, float* iou4, b200trk_stream_t stream) {
     B200_REQUIRE(net && (iou3 || iou4), "net_iou_from_arena: null pointer");
@@ -342,10 +443,7 @@ extern "C" int b200trk_net_iou_from_arena(b200trk_net_t* net, int S, float* iou3
     for (const Op& op : net->ops) {
         if (!op.iou) continue;
         if (op.kind == OP_CONV) {
-            if (op.tc) { if (int e = tc_conv_launch(net, op, S, st)) return e; continue; }
-            ConvShape sh{S, op.Hin, op.Win, op.Cin, op.Hout, op.Wout, op.Cout, op.k, op.stride, op.pad};
-            ConvEpilogue ep{op.bias, nullptr, op.relu};
-            if (int e = launch_conv_fp32(net->bufs[op.in], op.w, net->bufs[op.out], sh, ep, net->splitk_ws, net->splitk_ws_floats, net->sms, st)) return e;
+            if (int e = conv_step(net, op, S, st)) return e;
         } else if (op.kind == OP_EXPORT_NCHW) {
             float* dst = op.export_slot == 2 ? iou3 : iou4;
             if (dst)
@@ -407,7 +505,7 @@ extern "C" int b200trk_net_forward_iou(b200trk_net_t* net, const float* crop, in
 static int net_forward_eager(b200trk_net_t* net, const float* crop, int S, float* layer2, float* layer3, float* clf, float* iou3,
                              float* iou4, cudaStream_t st) {
     for (const Op& op : net->ops) {
-        if (op.iou && !iou3 && !iou4) continue;
+        if (op.init || (op.iou && !iou3 && !iou4)) continue;
         switch (op.kind) {
         case OP_PREPROCESS:
             if (int e = launch_preprocess(crop, net->bufs[op.out], S, op.Hin, op.Win, st)) return e;
@@ -418,17 +516,9 @@ static int net_forward_eager(b200trk_net_t* net, const float* crop, int S, float
         case OP_MAXPOOL:
             if (int e = launch_maxpool3x3s2(net->bufs[op.in], net->bufs[op.out], S, op.Hin, op.Win, op.Cin, st)) return e;
             break;
-        case OP_CONV: {
-            if (op.tc) {
-                if (int e = tc_conv_launch(net, op, S, st)) return e;
-                break;
-            }
-            ConvShape sh{S, op.Hin, op.Win, op.Cin, op.Hout, op.Wout, op.Cout, op.k, op.stride, op.pad};
-            ConvEpilogue ep{op.bias, op.res >= 0 ? net->bufs[op.res] : nullptr, op.relu};
-            if (int e = launch_conv_fp32(net->bufs[op.in], op.w, net->bufs[op.out], sh, ep, net->splitk_ws,
-                                         net->splitk_ws_floats, net->sms, st)) return e;
+        case OP_CONV:
+            if (int e = conv_step(net, op, S, st)) return e;
             break;
-        }
         case OP_EXPORT_NCHW: {
             float* dst = op.export_slot == 0 ? layer2 : op.export_slot == 1 ? layer3 : op.export_slot == 2 ? iou3 : iou4;
             if (dst)
@@ -439,6 +529,8 @@ static int net_forward_eager(b200trk_net_t* net, const float* crop, int S, float
             if (clf)
                 if (int e = launch_l2norm_nhwc_to_nchw(net->bufs[op.in], clf, net->l2_partials, S, op.Hin * op.Win, op.Cin,
                                                        net->norm_scale, 1e-5f, st)) return e;
+            break;
+        case OP_NCHW_IMPORT:
             break;
         }
     }

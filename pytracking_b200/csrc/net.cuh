@@ -6,7 +6,7 @@
 
 namespace b200trk {
 
-enum OpKind { OP_PREPROCESS, OP_STEM, OP_MAXPOOL, OP_CONV, OP_EXPORT_NCHW, OP_L2NORM_EXPORT };
+enum OpKind { OP_PREPROCESS, OP_STEM, OP_MAXPOOL, OP_CONV, OP_EXPORT_NCHW, OP_L2NORM_EXPORT, OP_NCHW_IMPORT };
 
 struct TcConv;   // tensor-core per-layer state (conv_tc.cu)
 
@@ -19,9 +19,28 @@ struct Op {
     float* bias = nullptr;   // device: [cout] or nullptr
     int export_slot = -1;    // OP_EXPORT_NCHW: 0 = layer2, 1 = layer3, 2 / 3 = the IoUNet features of layer2 / layer3
     int iou = 0;             // belongs to the IoUNet feature branch (skipped when no IoU output is requested)
+    int init = 0;            // belongs to a first-frame head (run by filter_init_conv / iou_ref_conv only, never by a forward pass)
     TcConv* tc = nullptr;
 };
 
+}  // namespace b200trk
+
+struct b200trk_net;
+struct b200trk_iou_modulation;
+
+namespace b200trk {
+// FilterInitializerLinear in two halves, so that a batch runs filter_conv once for all its images and pools each sequence's box apart:
+// filter_conv on the S normalised classification feature maps clf [S,C,H,W] (net.cu), then PrRoIPool of box r [x,y,w,h] on image
+// images[r] and the mean over the n boxes into filter [1,C,k,k] (init_heads.cu).
+int filter_init_conv(b200trk_net* net, const float* clf, int S, cudaStream_t st);
+int launch_nchw_to_nhwc(const float* in, float* out, int S, int HW, int C, cudaStream_t st);
+int filter_init_pool(b200trk_net* net, int S, int n, const int* images, const float* boxes, float* filter, cudaStream_t st);
+// AtomIoUNet's reference branch (conv3_1r on layer2, conv4_1r on layer3) on the activations the last forward pass of batch S left in
+// the arena, exported NCHW to net->iouref.nchw[0 / 1] for get_modulation's PrRoIPool (net.cu)
+int iou_ref_conv(b200trk_net* net, int S, cudaStream_t st);
+// get_modulation's pooling and linear blocks after iou_ref_conv: box r [x,y,w,h] of image images[r] -> mod3 [R,M3], mod4 [R,M4] (init_heads.cu)
+int iou_modulation_pool(b200trk_iou_modulation* m, b200trk_net* net, int S, int R, const int* images, const float* boxes, float* mod3,
+                        float* mod4, cudaStream_t st);
 }  // namespace b200trk
 
 struct b200trk_net {
@@ -36,6 +55,11 @@ struct b200trk_net {
     int dims[9] = {0};
     int feat_buf[2] = {-1, -1}, feat_hw[2][3] = {{0, 0, 0}, {0, 0, 0}};   // NHWC buffers / (C,H,W) of layer2 and layer3
     int iou_dims[6] = {0};               // IoUNet feature geometry {C,H,W} x 2 once b200trk_net_attach_iou_head ran
+    // FilterInitializerLinear once b200trk_net_attach_filter_init ran: plan steps of the NCHW import and filter_conv, the buffer of
+    // filter_conv's NCHW copy (PrRoIPool's layout), the filter size, filter_norm / pool_square, and device scratch
+    struct { int import_op = -1, conv_op = -1, nchw = -1, ksz = 0, norm = 0, square = 0; float *rois = nullptr, *pooled = nullptr; } finit;
+    // AtomIoUNet's conv3_1r / conv4_1r once b200trk_net_attach_iou_ref ran: their plan steps, NCHW output buffers and geometry {C,H,W}
+    struct { int op[2] = {-1, -1}, nchw[2] = {-1, -1}, dims[6] = {0, 0, 0, 0, 0, 0}; } iouref;
     double flops = 0.0;
     int sms = 1;
     // CUDA-graph cache of one forward pass (the per-frame call repeats with identical pointers): key + executable graph

@@ -111,6 +111,44 @@ class BackboneEngine:
         self.flops = _lib.lib().b200trk_net_flops(self.handle)
         del keep
 
+    def attach_iou_ref(self, state_dict, prefix="bb_regressor."):
+        """AtomIoUNet's conv3_1r / conv4_1r (atom_iou_net.py:30-35) as plan steps for get_modulation (iou.IoUModulation)."""
+        keep, descs = [], []
+        for name in ("conv3_1r", "conv4_1r"):
+            q = prefix + name
+            descs.append(_conv_entry(state_dict, keep, q + ".0.weight", q + ".1", 1, 1, bias_key=q + ".0.bias"))
+        arr = (_lib.ConvDesc * 2)(*descs)
+        with torch.cuda.device(self.device):
+            _lib.check(_lib.lib().b200trk_net_attach_iou_ref(self.handle, arr), "net_attach_iou_ref")
+        self.has_iou_ref = True
+        del keep
+
+    def attach_filter_init(self, state_dict, filter_size=4, filter_norm=False, pool_square=False,
+                           prefix="classifier.filter_initializer."):
+        """FilterInitializerLinear (initializer.py:118-173) from the state_dict's filter_conv; `filter_norm` / `pool_square` are its
+        constructor arguments (init_filter_norm / init_pool_square of dimpnet50 / klcedimpnet50, both False there)."""
+        keep = []
+        d = _conv_entry(state_dict, keep, prefix + "filter_conv.weight", None, 1, state_dict[prefix + "filter_conv.weight"].shape[-1] // 2,
+                        bias_key=prefix + "filter_conv.bias")
+        with torch.cuda.device(self.device):
+            _lib.check(_lib.lib().b200trk_net_attach_filter_init(self.handle, C.byref(d), int(filter_size), int(bool(filter_norm)),
+                                                                 int(bool(pool_square))), "net_attach_filter_init")
+        self.filter_size = int(filter_size)
+        del keep
+
+    def filter_init(self, clf, boxes, images=None):
+        """FilterInitializerLinear.forward: clf [S,C,H,W] normalised classification features (CUDA), boxes [n,4] (x, y, w, h), box r on
+        image images[r] (default r) -> filter [1,C,k,k], the mean over the n boxes."""
+        clf = clf.contiguous()
+        b = torch.as_tensor(boxes, dtype=torch.float32).reshape(-1, 4).contiguous().cpu()
+        img = None if images is None else (C.c_int * b.shape[0])(*[int(i) for i in images])
+        k = self.filter_size
+        out = torch.empty(1, clf.shape[1], k, k, device=clf.device, dtype=torch.float32)
+        _lib.check(_lib.lib().b200trk_net_filter_init(self.handle, C.c_void_p(clf.data_ptr()), int(clf.shape[0]), int(b.shape[0]),
+                                                      img, C.c_void_p(b.data_ptr()), C.c_void_p(out.data_ptr()),
+                                                      C.c_void_p(torch.cuda.current_stream(clf.device).cuda_stream)), "net_filter_init")
+        return out
+
     def iou_features(self, s):
         """get_iou_feat on the activations of the last forward pass (batch s) still in the arena -> (iou3, iou4)."""
         dev = self.device

@@ -113,13 +113,28 @@ def optimizer_args(state_dict, newton):
     return args, step_length, reg_weight
 
 
+FILTER_INITS = ("zero", "network")
+
+
+def attach_filter_init(backbone, state_dict, filter_init, filter_size, filter_norm, pool_square):
+    """The first-frame filter the online optimiser starts from.  "zero": FilterInitializerZero, what the reference uses under the
+    filter_init_zero parameter.  "network": the network's own FilterInitializerLinear (classifier.filter_initializer.filter_conv), what
+    the reference uses otherwise; filter_norm / pool_square are its constructor arguments (init_filter_norm / init_pool_square)."""
+    if filter_init not in FILTER_INITS:
+        raise ValueError("b200trk: filter_init=%r (one of %s)" % (filter_init, ", ".join(FILTER_INITS)))
+    if filter_init == "network":
+        backbone.attach_filter_init(state_dict, filter_size, filter_norm, pool_square)
+
+
 class DiMPFrameEngine:
     def __init__(self, state_dict, arch="resnet50", filter_size=4, memory_size=50, max_batch=1, crop_size=288, precision=0, device=None,
-                 newton=None):
+                 newton=None, filter_init="zero", init_filter_norm=False, init_pool_square=False):
         """newton: None for DiMP (DiMPSteepestDescentGN over the three LUTs of the state_dict), or a dict of
         PrDiMPSteepestDescentNewton constructor arguments (tracker.NEWTON_DEFAULTS names) for PrDiMP; the GN keys are then not read.
-        A state_dict that carries the optimiser's learnt log_step_length / filter_reg (a trained PrDiMP net) supplies those two."""
+        A state_dict that carries the optimiser's learnt log_step_length / filter_reg (a trained PrDiMP net) supplies those two.
+        filter_init: see attach_filter_init."""
         self.backbone = BackboneEngine(state_dict, arch, filter_size, max_batch, crop_size, precision, device)
+        attach_filter_init(self.backbone, state_dict, filter_init, filter_size, init_filter_norm, init_pool_square)
         self.device = self.backbone.device
         self.memory_size, self.filter_size, self.max_batch = memory_size, filter_size, max_batch
         if newton is not None:

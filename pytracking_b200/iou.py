@@ -9,6 +9,68 @@ import torch
 from . import _lib
 
 
+class IoUModulation:
+    """AtomIoUNet.get_modulation (atom_iou_net.py:138-170) after conv3_1r / conv4_1r (BackboneEngine.attach_iou_ref): the fc3_1r,
+    fc34_3r and fc34_4r blocks of the bb_regressor's state_dict, BN folded at create time."""
+
+    def __init__(self, state_dict, prefix="bb_regressor.", device=None):
+        if not torch.cuda.is_available():
+            raise RuntimeError("IoUModulation: CUDA device required (the engine has no CPU path)")
+        self.device = torch.device("cuda", torch.cuda.current_device()) if device is None else torch.device(device)
+        keep = []
+
+        def hp(key):
+            t = state_dict[prefix + key].detach().float().contiguous().cpu()
+            keep.append(t)
+            return t
+
+        def block(name):
+            w = hp(name + ".0.weight")
+            b = _lib.LinearBlock(w.data_ptr(), hp(name + ".0.bias").data_ptr(), hp(name + ".1.weight").data_ptr(),
+                                 hp(name + ".1.bias").data_ptr(), hp(name + ".1.running_mean").data_ptr(),
+                                 hp(name + ".1.running_var").data_ptr())
+            return b, w.shape
+        b31, s31 = block("fc3_1r")
+        b3, s3 = block("fc34_3r")
+        b4, s4 = block("fc34_4r")
+        self.C3 = int(state_dict[prefix + "conv3_1r.0.weight"].shape[0])
+        self.C4 = int(state_dict[prefix + "conv4_1r.0.weight"].shape[0])
+        self.D, self.M3, self.M4 = int(s31[0]), int(s3[0]), int(s4[0])
+        if tuple(s31[1:]) != (self.C3, 3, 3) or s3[1] != self.D + self.C4 or s4[1] != self.D + self.C4:
+            raise RuntimeError("IoUModulation: unexpected bb_regressor shapes %s %s %s" % (tuple(s31), tuple(s3), tuple(s4)))
+        h = C.c_void_p()
+        with torch.cuda.device(self.device):
+            _lib.check(_lib.lib().b200trk_iou_modulation_create(C.byref(h), C.byref(b31), C.byref(b3), C.byref(b4), self.C3, self.C4,
+                                                                self.D, self.M3, self.M4), "iou_modulation_create")
+        self.handle = h
+        del keep
+
+    def get(self, backbone, s, boxes, images=None):
+        """get_modulation of boxes [R,4] (x, y, w, h; box r on image images[r], default r) on the layer2 / layer3 activations of the last
+        forward pass (batch s) of `backbone` -> (mod3 [R,M3], mod4 [R,M4]) CUDA tensors."""
+        b = torch.as_tensor(boxes, dtype=torch.float32).reshape(-1, 4).contiguous().cpu()
+        R = b.shape[0]
+        img = None if images is None else (C.c_int * R)(*[int(i) for i in images])
+        m3 = torch.empty(R, self.M3, device=self.device, dtype=torch.float32)
+        m4 = torch.empty(R, self.M4, device=self.device, dtype=torch.float32)
+        _lib.check(_lib.lib().b200trk_iou_modulation_get(self.handle, backbone.handle, int(s), R, img, C.c_void_p(b.data_ptr()),
+                                                         C.c_void_p(m3.data_ptr()), C.c_void_p(m4.data_ptr()),
+                                                         C.c_void_p(torch.cuda.current_stream(self.device).cuda_stream)),
+                   "iou_modulation_get")
+        return m3, m4
+
+    def close(self):
+        if getattr(self, "handle", None):
+            _lib.lib().b200trk_iou_modulation_destroy(self.handle)
+            self.handle = None
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+
 class IoUPredictor:
     def __init__(self, state_dict, prefix="bb_regressor.", device=None):
         if not torch.cuda.is_available():

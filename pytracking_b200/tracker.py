@@ -197,13 +197,18 @@ class DiMPTracker(HostLogic):
     """initialize / track on one GPU.  `state_dict`: the DiMP network's state_dict (reference key names).
     `newton`: None for DiMP; for PrDiMP the PrDiMPSteepestDescentNewton constructor arguments (NEWTON_DEFAULTS names), to which
     params.filter_reg / softmax_reg / label_threshold / label_shrink apply as in DiMP._overwrite_classifier_params.  The localisation's
-    softmax then uses the optimiser's softmax_reg, as localize_target does (dimp.py:207)."""
+    softmax then uses the optimiser's softmax_reg, as localize_target does (dimp.py:207).
+    `filter_init`: the filter `initialize` starts the optimiser from -- "zero" (FilterInitializerZero, the reference under
+    filter_init_zero) or "network" (the network's FilterInitializerLinear, the reference otherwise; `init_filter_norm` /
+    `init_pool_square` are its constructor arguments, False in dimpnet50 and klcedimpnet50)."""
 
-    def __init__(self, state_dict, params=None, arch="resnet50", precision=0, device=None, newton=None, **param_overrides):
+    def __init__(self, state_dict, params=None, arch="resnet50", precision=0, device=None, newton=None, filter_init="zero",
+                 init_filter_norm=False, init_pool_square=False, **param_overrides):
         self.params, newton = tracker_settings(params, newton, **param_overrides)
         p = self.params
         self.engine = DiMPFrameEngine(state_dict, arch=arch, filter_size=4, memory_size=p.sample_memory_size, max_batch=1,
-                                      crop_size=p.image_sample_size, precision=precision, device=device, newton=newton)
+                                      crop_size=p.image_sample_size, precision=precision, device=device, newton=newton,
+                                      filter_init=filter_init, init_filter_norm=init_filter_norm, init_pool_square=init_pool_square)
         self.device = self.engine.device
         h = C.c_void_p()
         with torch.cuda.device(self.device):
@@ -233,18 +238,37 @@ class DiMPTracker(HostLogic):
                        "dimp_tracker_initialize_host")
         return {}
 
-    def attach_iounet(self, state_dict, modulation):
-        """IoUNet refinement: `state_dict` of the whole DiMP network (bb_regressor.* keys), `modulation` = the two modulation vectors
-        of the first-frame target (AtomIoUNet.get_modulation; DiMP.init_iou_net dimp.py:509-540)."""
-        from .iou import IoUPredictor
-        if not getattr(self.engine.backbone, "iou_dims", None):
-            self.engine.backbone.attach_iou_head(state_dict)
-        self.iou = IoUPredictor(state_dict, device=self.device)
-        m3 = modulation[0].detach().float().reshape(-1).cpu().contiguous()
-        m4 = modulation[1].detach().float().reshape(-1).cpu().contiguous()
+    def attach_iounet(self, state_dict, modulation=None):
+        """IoUNet refinement: `state_dict` of the whole DiMP network (bb_regressor.* keys).  `modulation`: the two modulation vectors
+        of the first-frame target (AtomIoUNet.get_modulation; DiMP.init_iou_net dimp.py:509-540), or None to compute them natively
+        from the bb_regressor's conv3_1r / conv4_1r / fc3_1r / fc34_*r weights during `initialize` (attach before it)."""
+        from .iou import IoUModulation, IoUPredictor
+        bb = self.engine.backbone
+        if not getattr(bb, "iou_dims", None):
+            bb.attach_iou_head(state_dict)
+        L = _lib.lib()
         with torch.cuda.device(self.device):
-            _lib.check(_lib.lib().b200trk_dimp_tracker_attach_iounet(self.handle, self.iou.handle, C.c_void_p(m3.data_ptr()),
-                                                                     C.c_void_p(m4.data_ptr())), "dimp_tracker_attach_iounet")
+            if modulation is None:
+                if not getattr(bb, "has_iou_ref", False):
+                    bb.attach_iou_ref(state_dict)
+                head = IoUModulation(state_dict, device=self.device)
+                _lib.check(L.b200trk_dimp_tracker_attach_modulation_head(self.handle, head.handle), "dimp_tracker_attach_modulation_head")
+                self.modulation_head = head            # the library holds the handle from here on
+                m3 = m4 = None
+            else:
+                m3 = modulation[0].detach().float().reshape(-1).cpu().contiguous()
+                m4 = modulation[1].detach().float().reshape(-1).cpu().contiguous()
+            pred = IoUPredictor(state_dict, device=self.device)
+            _lib.check(L.b200trk_dimp_tracker_attach_iounet(self.handle, pred.handle, None if m3 is None else C.c_void_p(m3.data_ptr()),
+                                                            None if m4 is None else C.c_void_p(m4.data_ptr())), "dimp_tracker_attach_iounet")
+            self.iou = pred
+
+    def modulation(self):
+        """(mod3, mod4) float32 numpy: the modulation vectors the IoUNet uses."""
+        m3, m4 = np.zeros(self.iou.C3, np.float32), np.zeros(self.iou.C4, np.float32)
+        _lib.check(_lib.lib().b200trk_dimp_tracker_modulation(self.handle, m3.ctypes.data_as(C.c_void_p), m4.ctypes.data_as(C.c_void_p)),
+                   "dimp_tracker_modulation")
+        return m3, m4
 
     @staticmethod
     def newton_from_reference(ref):
@@ -316,6 +340,9 @@ class DiMPTracker(HostLogic):
         if getattr(self, "iou", None) is not None:
             self.iou.close()
             self.iou = None
+        if getattr(self, "modulation_head", None) is not None:
+            self.modulation_head.close()
+            self.modulation_head = None
         if getattr(self, "engine", None) is not None:
             self.engine.close()
             self.engine = None
