@@ -589,6 +589,42 @@ int b200trk_dimp_tracker_initialize_host(b200trk_dimp_tracker_t* t, const uint8_
 /* Scalar half of initialize only (no device work): used by initialize_host and by the CPU tests. */
 int b200trk_dimp_tracker_init_state(b200trk_dimp_tracker_t* t, int H, int W, const double init_bbox[4], b200trk_crop_geom_t* init_crop,
                                     float init_target_box[4]);
+/* First-frame augmentation of DiMP.initialize (generate_init_samples / init_classifier, dimp.py:331-408, 536-575;
+ * pytracking/features/augmentation.py). Each transform reads the expanded patch (augmentation_expansion_factor x image_sample_size)
+ * and ends with crop_to_output: a replicate-clamped crop of image_sample_size centred on the patch and moved by `shift`. The caller
+ * supplies every random draw: the shifts of the flip / blur / rotate transforms and the dropout multipliers. */
+#define B200TRK_AUG_MAX 16                 /* samples of one augmented initialisation: transforms + dropout copies */
+enum { B200TRK_AUG_IDENTITY = 0, B200TRK_AUG_TRANSLATION = 1, B200TRK_AUG_FLIPLR = 2, B200TRK_AUG_BLUR = 3, B200TRK_AUG_ROTATE = 4,
+       B200TRK_AUG_SCALE = 5 /* augmentation.Scale: refused */ };
+typedef struct {
+    int    kind;              /* B200TRK_AUG_* */
+    int    shift[2];          /* Transform.shift (row, column) in pixels: the translation itself, or the random shift */
+    double param[2];          /* BLUR: sigma (row, column), at most 8; ROTATE: param[0] = angle in degrees */
+} b200trk_aug_transform_t;
+typedef struct {
+    int num_transforms;       /* T >= 1; transform[0] must be an IDENTITY without shift (the reference always puts it first) */
+    b200trk_aug_transform_t transform[B200TRK_AUG_MAX];
+    int num_dropout;          /* copies of sample 0's classification features ('dropout': (num, p)); T + num_dropout <= 16 */
+    const float* dropout_mult;   /* HOST [num_dropout, C]: F.dropout2d's per-channel multipliers, 0 or 1/(1-p) */
+} b200trk_dimp_augment_t;
+
+/* The T transformed crops of one expanded patch. patch: DEVICE [3, in_h, in_w] float32; crops: DEVICE [T, 3, out_h, out_w].
+ * Translation and flip are copies, rotation is cv2.warpAffine's fixed-point bilinear interpolation (bit for bit), blur a
+ * separable zero-padded convolution summed in tap order. */
+int b200trk_augment_crops(const float* patch, int in_h, int in_w, int out_h, int out_w, const b200trk_aug_transform_t* transforms, int T,
+                          float* crops, b200trk_stream_t stream);
+/* Host half of the augmented initialize (no device work): init_state, then the T + num_dropout target boxes init_target_boxes writes
+ * (target_boxes [T + num_dropout][4]), sample weights 1/(T + num_dropout) and num_init = num_stored = T + num_dropout. init_crop is
+ * the expanded patch's geometry, as init_state gives it. */
+int b200trk_dimp_tracker_init_state_augmented(b200trk_dimp_tracker_t* t, int H, int W, const double init_bbox[4],
+                                              const b200trk_dimp_augment_t* aug, b200trk_crop_geom_t* init_crop, float* target_boxes);
+/* DiMP.initialize with first-frame augmentation: the expanded patch, the T crops in one launch, the network at batch T, the
+ * dropout copies, the initial filter over all samples (the learnt initialiser when attached, else zero), every sample inserted
+ * with its box and weight, net_opt_iter iterations of the state's optimiser, and -- with a modulation head attached -- the IoUNet
+ * modulation of image 0 at its box (iounet_augmentation = False). Refused, before any state changes: more than 16 samples, a network
+ * built for batches smaller than T + num_dropout, the 'scale' transform, border_mode 'inside' and a tracker that is a batch slot. */
+int b200trk_dimp_tracker_initialize_augmented_host(b200trk_dimp_tracker_t* t, const uint8_t* image, int H, int W, const double init_bbox[4],
+                                                   const b200trk_dimp_augment_t* aug, b200trk_stream_t stream);
 /* Adopt the state of a tracker initialised elsewhere (e.g. the reference's DiMP.initialize with its augmentations, run above the
  * plug-in): the scalars, the host-side sample weights and counters. The device memory / boxes / filter are written by the caller
  * through the b200trk_dimp_state_* views. frame_num = the reference's self.frame_num. */

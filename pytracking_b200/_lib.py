@@ -79,6 +79,21 @@ class FrameInfo(C.Structure):
                 ("loc", LocResult), ("crop", CropGeom), ("refined", C.c_int), ("predicted_iou", C.c_float)]
 
 
+AUG_MAX = 16
+AUG_KINDS = {"identity": 0, "translation": 1, "fliplr": 2, "blur": 3, "rotate": 4, "scale": 5}
+
+
+class AugTransform(C.Structure):
+    """b200trk_aug_transform_t"""
+    _fields_ = [("kind", C.c_int), ("shift", C.c_int * 2), ("param", C.c_double * 2)]
+
+
+class DimpAugment(C.Structure):
+    """b200trk_dimp_augment_t"""
+    _fields_ = [("num_transforms", C.c_int), ("transform", AugTransform * AUG_MAX), ("num_dropout", C.c_int),
+                ("dropout_mult", C.c_void_p)]
+
+
 class BatchItem(C.Structure):
     """b200trk_batch_item_t"""
     _fields_ = [("slot", C.c_int), ("image", C.c_void_p), ("H", C.c_int), ("W", C.c_int), ("init", C.c_int), ("init_bbox", C.c_double * 4)]
@@ -174,6 +189,10 @@ SIGNATURES = {
     "b200trk_dimp_tracker_create": (_I, [C.POINTER(_VP), _VP, C.POINTER(DimpParams)]),
     "b200trk_dimp_tracker_destroy": (_I, [_VP]),
     "b200trk_dimp_tracker_initialize_host": (_I, [_VP, _VP, _I, _I, C.POINTER(C.c_double * 4), _VP]),
+    "b200trk_augment_crops": (_I, [_VP, _I, _I, _I, _I, C.POINTER(AugTransform), _I, _VP, _VP]),
+    "b200trk_dimp_tracker_init_state_augmented": (_I, [_VP, _I, _I, C.POINTER(C.c_double * 4), C.POINTER(DimpAugment), C.POINTER(CropGeom),
+                                                       _VP]),
+    "b200trk_dimp_tracker_initialize_augmented_host": (_I, [_VP, _VP, _I, _I, C.POINTER(C.c_double * 4), C.POINTER(DimpAugment), _VP]),
     "b200trk_dimp_tracker_init_state": (_I, [_VP, _I, _I, C.POINTER(C.c_double * 4), C.POINTER(CropGeom), C.POINTER(C.c_float * 4)]),
     "b200trk_dimp_tracker_adopt": (_I, [_VP, _I, _I, C.POINTER(C.c_float * 2), C.POINTER(C.c_float * 2), _F, C.POINTER(C.c_float * 2),
                                         _F, _F, _VP, _I, _I, _I, _I]),

@@ -20,10 +20,13 @@ from .tracker import frame_pointer, tracker_settings
 class DiMPBatchTracker:
     """`state_dict`, `params`, `arch`, `newton` as for `DiMPTracker` (newton=None: DiMP's GN optimiser; a dict: PrDiMP's Newton
     optimiser, whose softmax_reg the localisation then uses), `filter_init`, `init_filter_norm`, `init_pool_square` as for
-    `DiMPTracker`.  use_iou_net must be False."""
+    `DiMPTracker`.  use_iou_net must be False.  The first frame is not augmented: `augmentation` must be None."""
 
     def __init__(self, state_dict, params, capacity, arch="resnet50", newton=None, device=None, precision=0, filter_init="zero",
-                 init_filter_norm=False, init_pool_square=False, **param_overrides):
+                 init_filter_norm=False, init_pool_square=False, augmentation=None, **param_overrides):
+        if augmentation is not None:
+            raise NotImplementedError("DiMPBatchTracker: first-frame augmentation is not supported in a batch (its forward pass runs one "
+                                      "crop per sequence, an augmented start needs 13); use DiMPTracker for augmented initialisation")
         self.params, newton = tracker_settings(params, newton, **param_overrides)
         p = self.params
         if p.use_iou_net:

@@ -96,6 +96,10 @@ struct b200trk_dimp_tracker {
     FrameUpload frames;
     b200trk_loc_result_t* loc_dev = nullptr;
     b200trk_loc_result_t* loc_host = nullptr;      // pinned
+    // augmented initialisation (allocated by its first call): launch table, dropout multipliers, expanded patch
+    void* aug_table = nullptr;
+    float *aug_mult = nullptr, *aug_patch = nullptr;
+    size_t aug_patch_cap = 0;
 };
 
 // torch's floor division of float32 tensors (aten/src/ATen/native/BinaryOps.h div_floor_floating) for a divisor b > 0
@@ -223,7 +227,8 @@ extern "C" int b200trk_dimp_tracker_destroy(b200trk_dimp_tracker_t* t) {
     if (!t) return 0;
     if (t->loc_dev) cudaFree(t->loc_dev);
     if (t->loc_host) cudaFreeHost(t->loc_host);
-    for (float* q : {t->mod3, t->mod4, t->iou3, t->iou4, t->boxes_dev}) if (q) cudaFree(q);
+    for (float* q : {t->mod3, t->mod4, t->iou3, t->iou4, t->boxes_dev, t->aug_mult, t->aug_patch}) if (q) cudaFree(q);
+    if (t->aug_table) cudaFree(t->aug_table);
     if (t->boxes_host) cudaFreeHost(t->boxes_host);
     delete t;
     return 0;
@@ -279,6 +284,45 @@ extern "C" int b200trk_dimp_tracker_init_state(b200trk_dimp_tracker_t* t, int H,
     t->sw[0] = 1.0f;
     t->num_init = 1; t->num_stored = 1; t->prev_replace_ind = -1;
     t->initialized = 1;
+    return 0;
+}
+
+// The refusals of an augmented initialisation; checked before anything changes
+static int augment_ok(const b200trk_dimp_tracker* t, const b200trk_dimp_augment_t* aug, const char* what) {
+    const int T = aug->num_transforms, n = T + aug->num_dropout;
+    B200_REQUIRE(T >= 1 && aug->num_dropout >= 0 && n <= B200TRK_AUG_MAX, "%s: %d transforms and %d dropout copies (at most %d samples)",
+                 what, T, aug->num_dropout, B200TRK_AUG_MAX);
+    B200_REQUIRE(n <= (int)t->sw.size(), "%s: %d first-frame samples, sample_memory_size=%d", what, n, (int)t->sw.size());
+    B200_REQUIRE(aug->num_dropout == 0 || aug->dropout_mult, "%s: dropout copies without multipliers", what);
+    B200_REQUIRE(aug->transform[0].kind == B200TRK_AUG_IDENTITY && aug->transform[0].shift[0] == 0 && aug->transform[0].shift[1] == 0,
+                 "%s: the first transform must be the identity without shift (the un-augmented sample)", what);
+    const char* why = b200trk::augment_refusal(aug->transform, T);
+    B200_REQUIRE(!why, "%s: %s", what, why);
+    if (t->st) {        // (border_mode 'inside' is refused by init_state, before it changes anything)
+        B200_REQUIRE(t->st->clf, "%s: the tracker is a slot of a batch, whose forward pass runs one crop per sequence", what);
+        B200_REQUIRE(t->st->max_batch >= n, "%s: the network was built for batches of %d, the augmentation has %d samples", what,
+                     t->st->max_batch, n);
+    }
+    return 0;
+}
+
+extern "C" int b200trk_dimp_tracker_init_state_augmented(b200trk_dimp_tracker_t* t, int H, int W, const double b[4],
+                                                         const b200trk_dimp_augment_t* aug, b200trk_crop_geom_t* init_crop, float* target_boxes) {
+    B200_REQUIRE(t && b && aug && target_boxes, "dimp_tracker_init_state_augmented: null pointer");
+    if (int e = augment_ok(t, aug, "dimp_tracker_init_state_augmented")) return e;
+    float box[4];
+    if (int e = b200trk_dimp_tracker_init_state(t, H, W, b, init_crop, box)) return e;
+    // init_target_boxes (dimp.py:399-408): classifier_target_box + [shift_x, shift_y, 0, 0]; the dropout copies carry transform 0's
+    const int T = aug->num_transforms, n = T + aug->num_dropout;
+    for (int k = 0; k < n; ++k) {
+        const int* s = aug->transform[k < T ? k : 0].shift;
+        float* o = target_boxes + 4 * k;
+        o[0] = box[0] + (float)s[1]; o[1] = box[1] + (float)s[0]; o[2] = box[2] + 0.f; o[3] = box[3] + 0.f;
+    }
+    // init_memory (dimp.py:410-427): n init samples of weight x.new_ones(1) / n
+    std::fill(t->sw.begin(), t->sw.end(), 0.f);
+    for (int k = 0; k < n; ++k) t->sw[k] = 1.0f / (float)n;
+    t->num_init = n; t->num_stored = n;
     return 0;
 }
 
@@ -670,6 +714,61 @@ extern "C" int b200trk_dimp_tracker_initialize_host(b200trk_dimp_tracker_t* t, c
     // layer2 / layer3 activations of this init pass; the mean over that one box is its own vectors
     if (t->mod_native)
         if (int e = b200trk_iou_modulation_get(t->mod_head, s->net, 1, 1, nullptr, box, t->mod3, t->mod4, stream)) return e;
+    B200_CHECK_CUDA(cudaStreamSynchronize(st));
+    return 0;
+}
+
+// DiMP.initialize with use_augmentation (generate_init_samples, init_classifier, init_iou_net; dimp.py:331-408, 509-602)
+extern "C" int b200trk_dimp_tracker_initialize_augmented_host(b200trk_dimp_tracker_t* t, const uint8_t* image, int H, int W,
+                                                              const double init_bbox[4], const b200trk_dimp_augment_t* aug,
+                                                              b200trk_stream_t stream) {
+    const char* what = "dimp_tracker_initialize_augmented_host";
+    B200_REQUIRE(t && image && init_bbox && aug, "%s: null pointer", what);
+    B200_REQUIRE(t->st, "%s: host-logic-only tracker (created without a device state)", what);
+    if (int e = filter_init_ok(t->st, what)) return e;
+    if (int e = augment_ok(t, aug, what)) return e;
+    cudaStream_t st = (cudaStream_t)stream;
+    b200trk_dimp_state* s = t->st;
+    const int T = aug->num_transforms, nd = aug->num_dropout, n = T + nd;
+    b200trk_crop_geom_t g; float boxes[4 * B200TRK_AUG_MAX];
+    if (int e = b200trk_dimp_tracker_init_state_augmented(t, H, W, init_bbox, aug, &g, boxes)) return e;
+    const size_t patch_floats = (size_t)3 * g.out_h * g.out_w, plane = (size_t)s->Cc * s->Hc * s->Wc;
+    if (!t->aug_table) B200_CHECK_CUDA(cudaMalloc(&t->aug_table, b200trk::augment_table_bytes()));
+    if (!t->aug_mult) B200_CHECK_CUDA(cudaMalloc((void**)&t->aug_mult, (size_t)B200TRK_AUG_MAX * s->Cc * sizeof(float)));
+    if (patch_floats > t->aug_patch_cap) {
+        if (t->aug_patch) B200_CHECK_CUDA(cudaFree(t->aug_patch));
+        t->aug_patch = nullptr; t->aug_patch_cap = 0;
+        B200_CHECK_CUDA(cudaMalloc((void**)&t->aug_patch, patch_floats * sizeof(float)));
+        t->aug_patch_cap = patch_floats;
+    }
+    if (int e = t->frames.upload(1, &image, &H, &W, st)) return e;
+    // the whole expanded patch (sample_patch_transformed's sample_patch), then every transform's crop into the state's crop buffer
+    g.win_r = g.win_c = 0;
+    if (int e = b200trk_sample_patch(image, H, W, &g, g.out_h, g.out_w, t->aug_patch, stream)) return e;
+    const int iss = t->p.image_sample_size;
+    if (int e = b200trk::augment_crops(aug->transform, T, g.out_h, g.out_w, iss, iss, t->aug_table, t->aug_patch, s->crop, st)) return e;
+    if (int e = b200trk_net_forward(s->net, s->crop, T, nullptr, nullptr, s->clf, stream)) return e;
+    if (nd > 0) {
+        B200_CHECK_CUDA(cudaMemcpyAsync(t->aug_mult, aug->dropout_mult, (size_t)nd * s->Cc * sizeof(float), cudaMemcpyHostToDevice, st));
+        if (int e = b200trk::feature_dropout(s->clf, T, nd, s->Cc, s->Hc * s->Wc, t->aug_mult, st)) return e;
+    }
+    // get_filter on all n samples: FilterInitializerLinear's filter_conv runs on every map, dropout copies included (it has a bias
+    // and mixes channels, so it does not commute with the dropout mask), and the mean pools each sample at its own box
+    if (s->net->finit.conv_op >= 0) {
+        if (int e = filter_init_conv(s->net, s->clf, n, st)) return e;
+        if (int e = filter_init_pool(s->net, n, n, nullptr, boxes, s->filter, st)) return e;
+    } else {
+        B200_CHECK_CUDA(cudaMemsetAsync(s->filter, 0, (size_t)s->Cc * s->ksz * s->ksz * sizeof(float), st));
+    }
+    // init_memory, then net_opt_iter iterations with sample_weight = None, which both optimisers read as 1/n per sample
+    B200_CHECK_CUDA(cudaMemsetAsync(s->sw, 0, (size_t)s->memory_size * sizeof(float), st));
+    const int num_iter = t->p.net_opt_iter > 0 ? t->p.net_opt_iter : 0;
+    for (int k = 0; k < n; ++k)
+        if (int e = dimp_state_insert(s, s->clf + plane * k, k, boxes + 4 * k, t->sw.data(), n, k == n - 1 ? num_iter : 0, st)) return e;
+    // init_iou_net without iounet_augmentation: get_modulation of image 0 (the identity sample) at its box, on the layer2 / layer3
+    // activations the batch-T pass left in the arena
+    if (t->mod_native)
+        if (int e = b200trk_iou_modulation_get(t->mod_head, s->net, 1, 1, nullptr, boxes, t->mod3, t->mod4, stream)) return e;
     B200_CHECK_CUDA(cudaStreamSynchronize(st));
     return 0;
 }

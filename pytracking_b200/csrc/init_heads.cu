@@ -13,8 +13,37 @@
 #include <vector>
 
 #include "init_heads_kernels.cuh"      // kFilterInitMax, nchw_to_nhwc_kernel, filter_rois_kernel, filter_mean_kernel, mod_linear_kernel
+#include "augment_kernels.cuh"         // AugArgs, aug_prepare, augment_crops_kernel, feature_dropout_kernel
 
 namespace b200trk {
+
+const char* augment_refusal(const b200trk_aug_transform_t* xf, int T) {
+    AugArgs a;
+    return aug_prepare(xf, T, 2, 2, 1, 1, &a);
+}
+
+size_t augment_table_bytes() { return sizeof(AugArgs); }
+
+int augment_crops(const b200trk_aug_transform_t* xf, int T, int in_h, int in_w, int out_h, int out_w, void* table, const float* patch,
+                  float* crops, cudaStream_t st) {
+    AugArgs a;
+    const char* why = aug_prepare(xf, T, in_h, in_w, out_h, out_w, &a);
+    B200_REQUIRE(!why, "augment_crops: %s", why);
+    // from pageable memory: the copy is staged before cudaMemcpyAsync returns, so `a` may go out of scope
+    B200_CHECK_CUDA(cudaMemcpyAsync(table, &a, sizeof(AugArgs), cudaMemcpyHostToDevice, st));
+    const dim3 grid((out_w + kAugTile - 1) / kAugTile, (out_h + kAugTile - 1) / kAugTile, T);
+    augment_crops_kernel<<<grid, dim3(32, 8), aug_smem_floats(a) * sizeof(float), st>>>((const AugArgs*)table, patch, crops);
+    B200_LAUNCH_CHECK();
+    return 0;
+}
+
+int feature_dropout(float* clf, int T, int num, int C, int HW, const float* mult, cudaStream_t st) {
+    const size_t n = (size_t)num * C * HW;
+    if (n == 0) return 0;
+    feature_dropout_kernel<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(clf, T, num, C, HW, mult);
+    B200_LAUNCH_CHECK();
+    return 0;
+}
 
 int launch_nchw_to_nhwc(const float* in, float* out, int S, int HW, int C, cudaStream_t st) {
     nchw_to_nhwc_kernel<<<dim3((HW + 31) / 32, (C + 31) / 32, S), dim3(32, 8), 0, st>>>(in, out, HW, C);
@@ -171,6 +200,20 @@ extern "C" int b200trk_iou_modulation_get(b200trk_iou_modulation_t* m, b200trk_n
     cudaStream_t st = (cudaStream_t)stream;
     if (int e = iou_ref_conv(net, S, st)) return e;
     return iou_modulation_pool(m, net, S, R, images, boxes, mod3, mod4, st);
+}
+
+extern "C" int b200trk_augment_crops(const float* patch, int in_h, int in_w, int out_h, int out_w, const b200trk_aug_transform_t* transforms,
+                                     int T, float* crops, b200trk_stream_t stream) {
+    B200_REQUIRE(patch && transforms && crops, "augment_crops: null pointer");
+    void* table = nullptr;
+    B200_CHECK_CUDA(cudaMalloc(&table, augment_table_bytes()));
+    cudaStream_t st = (cudaStream_t)stream;
+    int e = augment_crops(transforms, T, in_h, in_w, out_h, out_w, table, patch, crops, st);
+    const cudaError_t ce = cudaStreamSynchronize(st);
+    cudaFree(table);
+    if (e) return e;
+    B200_REQUIRE(ce == cudaSuccess, "augment_crops: %s", cudaGetErrorString(ce));
+    return 0;
 }
 
 extern "C" int b200trk_net_filter_init_attached(const b200trk_net_t* net) { return net && net->finit.conv_op >= 0 ? 1 : 0; }

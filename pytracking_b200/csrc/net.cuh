@@ -41,6 +41,14 @@ int iou_ref_conv(b200trk_net* net, int S, cudaStream_t st);
 // get_modulation's pooling and linear blocks after iou_ref_conv: box r [x,y,w,h] of image images[r] -> mod3 [R,M3], mod4 [R,M4] (init_heads.cu)
 int iou_modulation_pool(b200trk_iou_modulation* m, b200trk_net* net, int S, int R, const int* images, const float* boxes, float* mod3,
                         float* mod4, cudaStream_t st);
+// The first-frame augmentation (init_heads.cu, augment_kernels.cuh): NULL or the reason a transform list is refused; the bytes of the
+// device launch table; the T crops [T,3,out_h,out_w] of patch [3,in_h,in_w] through `table`; the num dropout copies of row 0 of
+// clf [T + num, C, HW] with the DEVICE multipliers mult [num, C].
+const char* augment_refusal(const b200trk_aug_transform_t* xf, int T);
+size_t augment_table_bytes();
+int augment_crops(const b200trk_aug_transform_t* xf, int T, int in_h, int in_w, int out_h, int out_w, void* table, const float* patch,
+                  float* crops, cudaStream_t st);
+int feature_dropout(float* clf, int T, int num, int C, int HW, const float* mult, cudaStream_t st);
 }  // namespace b200trk
 
 struct b200trk_net {

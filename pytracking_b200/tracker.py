@@ -123,6 +123,58 @@ def tracker_settings(params, newton, **param_overrides):
     return p, newton
 
 
+def augmentation_from_params(tp):
+    """(augmentation, random_shift_factor) for DiMPTracker from a reference `TrackerParams`: params.augmentation when
+    use_augmentation is set (absent means set, as generate_init_samples reads it), else (None, 0.0) -- the un-augmented start."""
+    if not getattr(tp, "use_augmentation", True) or getattr(tp, "augmentation", None) is None:
+        return None, 0.0
+    return dict(tp.augmentation), float(getattr(tp, "random_shift_factor", 0) or 0)
+
+
+def augmentation_samples(augmentation):
+    """First-frame samples an augmentation dict gives: the identity, its transforms and its dropout copies."""
+    a = augmentation
+    if "scale" in a:
+        raise NotImplementedError("b200trk: augmentation 'scale' is not implemented (no DiMP-family parameter file uses it)")
+    return (1 + len(a.get("shift", [])) + len(a.get("relativeshift", [])) + int(bool(a.get("fliplr"))) + len(a.get("blur", [])) +
+            len(a.get("rotate", [])) + int(a.get("dropout", (0, 0))[0]))
+
+
+def draw_augmentation(augmentation, image_sample_size, random_shift_factor, feature_dim):
+    """The b200trk_dimp_augment_t of one augmented initialisation, with every random number drawn as the reference draws it
+    (generate_init_samples, dimp.py:364-388, then init_classifier's dropout, dimp.py:544-547) from torch's CPU generator: the flip,
+    blur and rotate shifts in that order, then F.dropout2d's masks -- drawn on ones [num, C, 1, 1], which consumes the generator
+    exactly as dropout2d on the features does.  -> (descriptor, multipliers tensor kept alive by the caller)."""
+    a = augmentation
+    augmentation_samples(a)
+    iss = torch.Tensor([image_sample_size, image_sample_size])
+    if random_shift_factor > 0:
+        rand_shift = lambda: ((torch.rand(2) - 0.5) * iss * random_shift_factor).long().tolist()
+    else:
+        rand_shift = lambda: [0, 0]
+    K = _lib.AUG_KINDS
+    xf = [(K["identity"], [0, 0], (0.0, 0.0))]
+    xf += [(K["translation"], [int(s[0]), int(s[1])], (0.0, 0.0)) for s in a.get("shift", [])]
+    xf += [(K["translation"], (torch.Tensor(s) * iss / 2).long().tolist(), (0.0, 0.0)) for s in a.get("relativeshift", [])]
+    if a.get("fliplr"):
+        xf.append((K["fliplr"], rand_shift(), (0.0, 0.0)))
+    for sg in a.get("blur", []):
+        xf.append((K["blur"], rand_shift(), tuple(float(v) for v in (sg if isinstance(sg, (tuple, list)) else (sg, sg)))))
+    for ang in a.get("rotate", []):
+        xf.append((K["rotate"], rand_shift(), (float(ang), 0.0)))
+    num, prob = a.get("dropout", (0, 0.0))
+    d = _lib.DimpAugment()
+    d.num_transforms = len(xf)
+    for k, (kind, shift, param) in enumerate(xf):
+        d.transform[k].kind, d.transform[k].shift[0], d.transform[k].shift[1] = kind, int(shift[0]), int(shift[1])
+        d.transform[k].param[0], d.transform[k].param[1] = param
+    mult = None
+    if int(num) > 0:
+        mult = torch.nn.functional.dropout2d(torch.ones(int(num), feature_dim, 1, 1), p=prob, training=True).reshape(int(num), -1).contiguous()
+        d.num_dropout, d.dropout_mult = int(num), mult.data_ptr()
+    return d, mult
+
+
 def frame_pointer(image, staging, key, who):
     """A uint8 [H,W,3] RGB frame -> (keep-alive, pointer, H, W, on_device).  A CUDA tensor or a pinned host tensor is used in place.
     Any other frame (ndarray, pageable tensor) is copied into the pinned buffer staging[key], which is reused while the frame size
@@ -155,6 +207,15 @@ class HostLogic:
         bb = (C.c_double * 4)(*[float(v) for v in init_bbox])
         _lib.check(_lib.lib().b200trk_dimp_tracker_init_state(self.handle, H, W, C.byref(bb), C.byref(g), C.byref(box)), "init_state")
         return g, np.array(box, dtype=np.float32)
+
+    def init_state_augmented(self, H, W, init_bbox, augment):
+        """Host half of the augmented initialize for a drawn descriptor (draw_augmentation) -> (crop geometry, target boxes [n,4])."""
+        n = augment.num_transforms + augment.num_dropout
+        g, boxes = _lib.CropGeom(), np.zeros((max(n, 1), 4), np.float32)
+        bb = (C.c_double * 4)(*[float(v) for v in init_bbox])
+        _lib.check(_lib.lib().b200trk_dimp_tracker_init_state_augmented(self.handle, H, W, C.byref(bb), C.byref(augment), C.byref(g),
+                                                                        boxes.ctypes.data_as(C.c_void_p)), "init_state_augmented")
+        return g, boxes[:n]
 
     def adopt(self, H, W, state9, sample_weights, num_stored, num_init, previous_replace_ind=-1, frame_num=1):
         s = [float(v) for v in state9]
@@ -200,13 +261,21 @@ class DiMPTracker(HostLogic):
     softmax then uses the optimiser's softmax_reg, as localize_target does (dimp.py:207).
     `filter_init`: the filter `initialize` starts the optimiser from -- "zero" (FilterInitializerZero, the reference under
     filter_init_zero) or "network" (the network's FilterInitializerLinear, the reference otherwise; `init_filter_norm` /
-    `init_pool_square` are its constructor arguments, False in dimpnet50 and klcedimpnet50)."""
+    `init_pool_square` are its constructor arguments, False in dimpnet50 and klcedimpnet50).
+    `augmentation`: None starts from the un-augmented first-frame sample; a dict in the form of the reference's params.augmentation
+    (with `random_shift_factor`, see augmentation_from_params) starts as DiMP.initialize does with use_augmentation: the transformed
+    crops, the dropout copies and a first optimisation over all of them.  The network is then sized for that many samples."""
 
     def __init__(self, state_dict, params=None, arch="resnet50", precision=0, device=None, newton=None, filter_init="zero",
-                 init_filter_norm=False, init_pool_square=False, **param_overrides):
+                 init_filter_norm=False, init_pool_square=False, augmentation=None, random_shift_factor=0.0, **param_overrides):
         self.params, newton = tracker_settings(params, newton, **param_overrides)
         p = self.params
-        self.engine = DiMPFrameEngine(state_dict, arch=arch, filter_size=4, memory_size=p.sample_memory_size, max_batch=1,
+        self.augmentation = None if augmentation is None else dict(augmentation)
+        self.random_shift_factor = float(random_shift_factor or 0.0)
+        n = 1 if self.augmentation is None else augmentation_samples(self.augmentation)
+        if n > _lib.AUG_MAX:
+            raise ValueError("DiMPTracker: the augmentation gives %d first-frame samples (at most %d)" % (n, _lib.AUG_MAX))
+        self.engine = DiMPFrameEngine(state_dict, arch=arch, filter_size=4, memory_size=p.sample_memory_size, max_batch=n,
                                       crop_size=p.image_sample_size, precision=precision, device=device, newton=newton,
                                       filter_init=filter_init, init_filter_norm=init_filter_norm, init_pool_square=init_pool_square)
         self.device = self.engine.device
@@ -230,12 +299,21 @@ class DiMPTracker(HostLogic):
         return keep, ptr, H, W
 
     def initialize(self, image, info):
-        """DiMP.initialize for the un-augmented configuration (see b200trk_dimp_tracker_initialize_host)."""
+        """DiMP.initialize: un-augmented (b200trk_dimp_tracker_initialize_host), or with the tracker's augmentation, whose random
+        numbers come from torch's CPU generator in the reference's order (draw_augmentation;
+        b200trk_dimp_tracker_initialize_augmented_host)."""
         keep, ptr, H, W = self._frame(image, False)
         bb = (C.c_double * 4)(*[float(v) for v in info["init_bbox"]])
+        L = _lib.lib()
         with torch.cuda.device(self.device):
-            _lib.check(_lib.lib().b200trk_dimp_tracker_initialize_host(self.handle, C.c_void_p(ptr), H, W, C.byref(bb), self._stream()),
-                       "dimp_tracker_initialize_host")
+            if self.augmentation is None:
+                _lib.check(L.b200trk_dimp_tracker_initialize_host(self.handle, C.c_void_p(ptr), H, W, C.byref(bb), self._stream()),
+                           "dimp_tracker_initialize_host")
+            else:
+                d, mult = draw_augmentation(self.augmentation, self.params.image_sample_size, self.random_shift_factor,
+                                            self.engine.feat_dims[0])
+                _lib.check(L.b200trk_dimp_tracker_initialize_augmented_host(self.handle, C.c_void_p(ptr), H, W, C.byref(bb), C.byref(d),
+                                                                            self._stream()), "dimp_tracker_initialize_augmented_host")
         return {}
 
     def attach_iounet(self, state_dict, modulation=None):
