@@ -335,7 +335,9 @@ typedef struct b200trk_transformer b200trk_transformer_t;
 
 /* Transformer (ltr/models/transformer/transformer.py:66-96; normalize_before=False, activation relu, eval mode) for a fixed
  * token count L and batch B (ToMP: L = (2 train + 1 test) * 18 * 18 = 972, B = 2 = {cls, bbreg}, d_model 256, 8 heads,
- * FF 2048; ltr/models/transformer/filter_predictor.py:92-150). head_dim must be 32. */
+ * FF 2048; ltr/models/transformer/filter_predictor.py:92-150). head_dim must be 32; L * B <= 65536, B <= 8, and L at most what the
+ * decoder's attention can hold in shared memory ((L + 256) floats: L <= 57792 on an H100); a larger L is refused before anything is
+ * allocated, with the limit in the message. */
 int b200trk_transformer_create(b200trk_transformer_t** out, const b200trk_enc_layer_t* enc, int n_enc,
                                const b200trk_dec_layer_t* dec, int n_dec, const float* dec_norm_weight,
                                const float* dec_norm_bias, int d_model, int nhead, int dim_ff, int L, int B);
@@ -346,6 +348,22 @@ int b200trk_transformer_destroy(b200trk_transformer_t* t);
 int b200trk_transformer_forward(b200trk_transformer_t* t, const float* src, const float* pos, int Bp,
                                 const unsigned char* key_padding_mask, const float* query_embed, float* hs, float* memory,
                                 b200trk_stream_t stream);
+/* Debug read-back (tests). A forward pass runs a fixed sequence of num_launches launches: per encoder layer 9 (add_pos, GEMM [q|k],
+ * GEMM v, attention, GEMM out_proj + residual, LayerNorm, GEMM linear1 + ReLU, GEMM linear2 + residual, LayerNorm), then add_pos of the
+ * memory, then per decoder layer 13 (small_linear v, small_linear out_proj + residual, LayerNorm, add_pos of the query, small_linear q,
+ * GEMM k, GEMM v, single-query attention, small_linear out_proj + residual, LayerNorm, small_linear linear1 + ReLU, small_linear
+ * linear2 + residual, LayerNorm), then the final LayerNorm into hs. Every launch writes a buffer it does not read.
+ * stop_after(k) makes later forward passes return right after launch k (hs / memory are then not written); -1 runs them to the end.
+ * debug_buffer copies internal buffer `buf` (DEVICE dst; NULL only reports the size) and reports its float count:
+ *   0 src, 1 qkin, 2 qk [L,B,2D], 3 v, 4 att, 5 tmp, 6 ff [L,B,FF], 7 mem_pos, 8 k      (encoder, [L,B,D] unless noted)
+ *   9 tgt, 10 t1, 11 t2, 12 q, 13 att, 14 ff [B,FF], 15 qpos                              (decoder, [B,D] unless noted)
+ * debug_gemm(g): GEMM g in execution order (5 per encoder layer: [q|k], v, out_proj, linear1, linear2; then 2 per decoder layer: k, v),
+ * each a 1x1 convolution over an Ht x Wt token image, as last launched: info = {in buffer, out buffer, residual buffer or -1, relu, Ht,
+ * Wt, K, N, grid.x, grid.y, grid.z (splits), BN, split-K reduction (as b200trk_net_op_splitk_reduction), tile width, tile height}. */
+int b200trk_transformer_debug_num_launches(const b200trk_transformer_t* t);
+int b200trk_transformer_debug_stop_after(b200trk_transformer_t* t, int launch);
+int b200trk_transformer_debug_buffer(const b200trk_transformer_t* t, int buf, float* dst, long long* floats, b200trk_stream_t stream);
+int b200trk_transformer_debug_gemm(const b200trk_transformer_t* t, int gemm, int info[15]);
 
 
 /* ToMP token assembly -- FilterPredictor.predict_cls_bbreg_filters_parallel up to the transformer call
@@ -368,6 +386,15 @@ int b200trk_tower_destroy(b200trk_tower_t* t);
 double b200trk_tower_flops(const b200trk_tower_t* t);
 /* feat DEVICE [S,C,H,W], attention DEVICE [S,H,W] (NULL = ones) -> out DEVICE [S,4,H,W] = exp(bbreg_layer(tower(attention * feat))). */
 int b200trk_tower_forward(b200trk_tower_t* t, const float* feat, const float* attention, int S, float* out, b200trk_stream_t stream);
+/* Debug read-back (tests). A forward pass runs 2 n_convs + 1 launches: the import, then per convolution i the convolution and (but for
+ * the last) GroupNorm + ReLU in place on its output, then the exp export. stop_after(k) makes later forward passes return right after
+ * launch k; -1 runs them to the end. debug_buffer copies activation buffer `buf` NHWC [S,H,W,C] (0 the imported input, i + 1 the output
+ * of convolution i: GroupNorm's input until it has run, its output after). debug_conv(i): info = {Cin, Cout, runs on the tensor cores,
+ * grid.x, grid.y, grid.z, BN, split-K reduction, tile width, output buffer}, the launch fields 0 on the fp32 CUDA-core path. */
+int b200trk_tower_debug_num_launches(const b200trk_tower_t* t);
+int b200trk_tower_debug_stop_after(b200trk_tower_t* t, int launch);
+int b200trk_tower_debug_buffer(const b200trk_tower_t* t, int buf, int S, float* dst, b200trk_stream_t stream);
+int b200trk_tower_debug_conv(const b200trk_tower_t* t, int conv, int info[10]);
 
 /* ------------------------------------------------------------------------------------------------
  * Native op -- Precise RoI Pooling (the reference's only CUDA component)

@@ -161,11 +161,19 @@ SIGNATURES = {
     "b200trk_transformer_create": (_I, [C.POINTER(_VP), C.POINTER(EncLayer), _I, C.POINTER(DecLayer), _I, _VP, _VP, _I, _I, _I, _I, _I]),
     "b200trk_transformer_destroy": (_I, [_VP]),
     "b200trk_transformer_forward": (_I, [_VP, _VP, _VP, _I, _VP, _VP, _VP, _VP, _VP]),
+    "b200trk_transformer_debug_num_launches": (_I, [_VP]),
+    "b200trk_transformer_debug_stop_after": (_I, [_VP, _I]),
+    "b200trk_transformer_debug_buffer": (_I, [_VP, _I, _VP, C.POINTER(C.c_longlong), _VP]),
+    "b200trk_transformer_debug_gemm": (_I, [_VP, _I, C.POINTER(C.c_int * 15)]),
     "b200trk_tomp_tokens": (_I, [_VP] * 13 + [_I, _I, _I, _I, _I, _I, _I, _VP]),
     "b200trk_tower_create": (_I, [C.POINTER(_VP), C.POINTER(ConvDesc), _I, C.POINTER(_VP), C.POINTER(_VP), _I, _I, _I, _I, _I]),
     "b200trk_tower_destroy": (_I, [_VP]),
     "b200trk_tower_flops": (C.c_double, [_VP]),
     "b200trk_tower_forward": (_I, [_VP, _VP, _VP, _I, _VP, _VP]),
+    "b200trk_tower_debug_num_launches": (_I, [_VP]),
+    "b200trk_tower_debug_stop_after": (_I, [_VP, _I]),
+    "b200trk_tower_debug_buffer": (_I, [_VP, _I, _I, _VP, _VP]),
+    "b200trk_tower_debug_conv": (_I, [_VP, _I, C.POINTER(C.c_int * 10)]),
     "b200trk_prroi_pool_forward": (_I, [_VP, _VP, _VP, _I, _I, _I, _I, _I, _I, _I, _F, _VP]),
     "b200trk_prroi_pool_backward": (_I, [_VP, _VP, _VP, _VP, _VP, _I, _I, _I, _I, _I, _I, _I, _F, _VP]),
     "b200trk_prroi_pool_coor_backward": (_I, [_VP, _VP, _VP, _VP, _VP, _I, _I, _I, _I, _I, _I, _I, _F, _VP]),

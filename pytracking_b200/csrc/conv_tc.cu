@@ -633,6 +633,10 @@ int tc_conv_grid(const Op& op, int dims[4]) {
     dims[0] = P.tiles_w * P.tiles_h * S; dims[1] = P.BN ? op.Cout / P.BN : 0; dims[2] = P.splits; dims[3] = P.BN;
     return 0;
 }
+int tc_conv_tile(const Op& op, int dims[2]) {
+    dims[0] = op.tc->P.BW; dims[1] = op.tc->P.BH;
+    return 0;
+}
 int tc_conv_reduction(const Op& op) {
     const TcParams& P = op.tc->P;
     return P.splits <= 1 ? 0 : P.cluster_red ? 1 : 2;

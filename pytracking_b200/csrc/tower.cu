@@ -25,6 +25,7 @@ struct b200trk_tower {
     b200trk_net net;             // weights / activation buffers / ops (OP_CONV only) owned like a network plan
     std::vector<float*> gamma, beta;
     int C = 0, H = 0, W = 0, in_buf = -1;
+    int stop_after = -1;         // debug: forward returns after this launch of its fixed sequence (-1: runs to the end)
 };
 
 extern "C" int b200trk_tower_destroy(b200trk_tower_t* t);
@@ -110,8 +111,11 @@ extern "C" int b200trk_tower_forward(b200trk_tower_t* t, const float* feat, cons
     cudaStream_t st = (cudaStream_t)stream;
     b200trk_net* net = &t->net;
     const int HW = t->H * t->W;
+    int launches = 0;
+    auto stop = [&]() { return launches++ == t->stop_after; };      // true right after the launch a debug run stops at
     import_scaled_kernel<<<dim3((HW + 31) / 32, (t->C + 31) / 32, S), dim3(32, 8), 0, st>>>(feat, attention, net->bufs[t->in_buf], HW, t->C);
     B200_LAUNCH_CHECK();
+    if (stop()) return 0;
     const int n = (int)net->ops.size();
     for (int i = 0; i < n; ++i) {
         const Op& op = net->ops[i];
@@ -122,14 +126,46 @@ extern "C" int b200trk_tower_forward(b200trk_tower_t* t, const float* feat, cons
             ConvEpilogue ep{op.bias, nullptr, 0};
             if (int e = launch_conv_fp32(net->bufs[op.in], op.w, net->bufs[op.out], sh, ep, net->splitk_ws, net->splitk_ws_floats, net->sms, st)) return e;
         }
+        if (stop()) return 0;
         if (i < n - 1) {
             groupnorm1_relu_kernel<<<S, 1024, 0, st>>>(net->bufs[op.out], t->gamma[i], t->beta[i], HW, op.Cout, 1e-5f);
             B200_LAUNCH_CHECK();
+            if (stop()) return 0;
         }
     }
     const Op& last = net->ops[n - 1];
     const int tot = S * HW * last.Cout;
     export_exp_kernel<<<(tot + 255) / 256, 256, 0, st>>>(net->bufs[last.out], out, HW, last.Cout, S);
     B200_LAUNCH_CHECK();
+    return 0;
+}
+
+// ---- debug read-back (tests): stop a forward pass after launch k, copy an activation buffer, report each convolution's launch plan ----
+namespace b200trk { int tc_conv_grid(const Op& op, int dims[4]); int tc_conv_reduction(const Op& op); int tc_conv_tile(const Op& op, int dims[2]); }
+
+extern "C" int b200trk_tower_debug_num_launches(const b200trk_tower_t* t) {
+    return t ? 2 * (int)t->net.ops.size() + 1 : 0;
+}
+
+extern "C" int b200trk_tower_debug_stop_after(b200trk_tower_t* t, int launch) {
+    B200_REQUIRE(t && launch >= -1 && launch < b200trk_tower_debug_num_launches(t), "tower_debug_stop_after: bad argument");
+    t->stop_after = launch;
+    return 0;
+}
+
+extern "C" int b200trk_tower_debug_buffer(const b200trk_tower_t* t, int buf, int S, float* dst, b200trk_stream_t stream) {
+    B200_REQUIRE(t && dst && buf >= 0 && buf < (int)t->net.bufs.size() && S >= 1 && S <= t->net.max_batch, "tower_debug_buffer: bad argument");
+    B200_CHECK_CUDA(cudaMemcpyAsync(dst, t->net.bufs[buf], (size_t)S * t->net.buf_floats[buf] * sizeof(float), cudaMemcpyDeviceToDevice,
+                                    (cudaStream_t)stream));
+    return 0;
+}
+
+extern "C" int b200trk_tower_debug_conv(const b200trk_tower_t* t, int conv, int info[10]) {
+    B200_REQUIRE(t && info && conv >= 0 && conv < (int)t->net.ops.size(), "tower_debug_conv: bad argument");
+    const Op& op = t->net.ops[conv];
+    int g[4] = {0, 0, 0, 0}, tile[2] = {0, 0}, red = 0;
+    if (op.tc) { tc_conv_grid(op, g); tc_conv_tile(op, tile); red = tc_conv_reduction(op); }
+    const int v[10] = {op.Cin, op.Cout, op.tc ? 1 : 0, g[0], g[1], g[2], g[3], red, tile[0], op.out};
+    memcpy(info, v, sizeof(v));
     return 0;
 }

@@ -38,6 +38,7 @@ struct b200trk_transformer {
     int b_src = -1, b_qkin = -1, b_qk = -1, b_v = -1, b_att = -1, b_tmp = -1, b_ff = -1, b_mem_pos = -1, b_k = -1;
     float *pos_full = nullptr;            // [L,B,D] broadcast copy of pos when Bp == 1 (not needed: add_pos handles Bp)
     float *d_tgt = nullptr, *d_t1 = nullptr, *d_t2 = nullptr, *d_q = nullptr, *d_att = nullptr, *d_ff = nullptr, *d_qpos = nullptr;
+    int stop_after = -1;                  // debug: forward returns after this launch of its fixed sequence (-1: runs to the end)
 };
 
 static int t_alloc(b200trk_transformer* t, float** p, size_t floats) {
@@ -91,6 +92,20 @@ extern "C" int b200trk_transformer_create(b200trk_transformer_t** out, const b20
     B200_REQUIRE(out && enc && dec && dec_norm_w && dec_norm_b, "transformer_create: null pointer");
     B200_REQUIRE(d_model % 64 == 0 && d_model / nhead == 32 && dim_ff % 64 == 0, "transformer_create: d_model=%d nhead=%d dim_ff=%d not supported (head_dim must be 32, widths multiples of 64)", d_model, nhead, dim_ff);
     B200_REQUIRE(L >= 1 && B >= 1 && B <= 8 && (size_t)L * B <= 65536, "transformer_create: L=%d B=%d out of range", L, B);
+    // attention_q1_kernel keeps all L scores of its (b, h) in dynamic shared memory, next to 8 x 32 partial outputs: above the default
+    // 48 KB it has to opt in, and the device's opt-in maximum caps L
+    cudaFuncAttributes q1;
+    int dev = 0, optin = 0;
+    B200_CHECK_CUDA(cudaFuncGetAttributes(&q1, attention_q1_kernel));
+    B200_CHECK_CUDA(cudaGetDevice(&dev));
+    B200_CHECK_CUDA(cudaDeviceGetAttribute(&optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, dev));
+    const int max_L = (optin - (int)q1.sharedSizeBytes) / (int)sizeof(float) - 8 * AT_HD;
+    B200_REQUIRE(L <= max_L, "transformer_create: L=%d above this device's limit L <= %d (the decoder's attention holds L + %d floats in "
+                 "shared memory, at most %d bytes with %d static)", L, max_L, 8 * AT_HD, optin, (int)q1.sharedSizeBytes);
+    const int q1_smem = (L + 8 * AT_HD) * (int)sizeof(float);
+    // the default 48 KB covers static + dynamic shared memory together; the attribute is never lowered (engines of a smaller L share it)
+    if (q1_smem + (int)q1.sharedSizeBytes > 48 * 1024 && q1.maxDynamicSharedSizeBytes < q1_smem)
+        B200_CHECK_CUDA(cudaFuncSetAttribute(attention_q1_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, q1_smem));
     b200trk_transformer* t = new b200trk_transformer();
     t->D = d_model; t->H = nhead; t->FF = dim_ff; t->L = L; t->B = B; t->n_enc = n_enc; t->n_dec = n_dec; t->M = L * B;
     t->box.max_batch = 1; t->box.precision = 0; t->box.sms = device_sm_count();
@@ -171,6 +186,8 @@ extern "C" int b200trk_transformer_forward(b200trk_transformer_t* t, const float
     cudaStream_t st = (cudaStream_t)stream;
     const int D = t->D, M = t->M, L = t->L, B = t->B, H = t->H, FF = t->FF;
     auto buf = [&](int id) { return t->box.bufs[id]; };
+    int launches = 0;
+    auto stop = [&]() { return launches++ == t->stop_after; };      // true right after the launch a debug run stops at
     const float scale = 1.0f / sqrtf(32.f);
     auto gemm = [&](int gid) { return tc_conv_launch(&t->box, t->gemms[gid], 1, st); };
     auto ln = [&](const float* x, const b200trk_transformer::LN& n, float* y, int T) {
@@ -194,17 +211,26 @@ extern "C" int b200trk_transformer_forward(b200trk_transformer_t* t, const float
     for (int i = 0; i < t->n_enc; ++i) {
         auto& E = t->enc[i];
         if (addpos(buf(t->b_src), buf(t->b_qkin))) { set_error("transformer: add_pos launch failed"); return 1; }
+        if (stop()) return 0;
         if (int e = gemm(E.g_qk)) return e;                              // [M, 2D] = (src + pos) [Wq; Wk]^T + b
+        if (stop()) return 0;
         if (int e = gemm(E.g_v)) return e;                               // [M, D]  = src Wv^T + b
+        if (stop()) return 0;
         attention_kernel<<<dim3((L + AT_Q - 1) / AT_Q, B * H), 128, 0, st>>>(buf(t->b_qk), buf(t->b_qk) + D, buf(t->b_v),
                                                                               key_padding_mask, buf(t->b_att), L, L, B, H, 2 * D,
                                                                               2 * D, D, D, scale);
         B200_LAUNCH_CHECK();
+        if (stop()) return 0;
         if (int e = gemm(E.g_o)) return e;                               // tmp = src + att Wo^T + b
+        if (stop()) return 0;
         if (ln(buf(t->b_tmp), E.n1, buf(t->b_src), M)) { set_error("transformer: layernorm launch failed"); return 1; }
+        if (stop()) return 0;
         if (int e = gemm(E.g_f1)) return e;                              // ff = relu(src W1^T + b1)
+        if (stop()) return 0;
         if (int e = gemm(E.g_f2)) return e;                              // tmp = src + ff W2^T + b2
+        if (stop()) return 0;
         if (ln(buf(t->b_tmp), E.n2, buf(t->b_src), M)) { set_error("transformer: layernorm launch failed"); return 1; }
+        if (stop()) return 0;
     }
     B200_CHECK_CUDA(cudaMemcpyAsync(memory, buf(t->b_src), (size_t)M * D * sizeof(float), cudaMemcpyDeviceToDevice, st));
     // ---------------- decoder (one query per batch element) ----------------
@@ -212,27 +238,83 @@ extern "C" int b200trk_transformer_forward(b200trk_transformer_t* t, const float
     B200_CHECK_CUDA(cudaMemsetAsync(t->d_tgt, 0, (size_t)B * D * sizeof(float), st));
     for (int b = 0; b < B; ++b)
         B200_CHECK_CUDA(cudaMemcpyAsync(t->d_qpos + (size_t)b * D, query_embed, D * sizeof(float), cudaMemcpyDeviceToDevice, st));
+    if (stop()) return 0;
     for (int i = 0; i < t->n_dec; ++i) {
         auto& Dl = t->dec[i];
         // self attention over a single token: softmax over one key is 1, so the output is out_proj(v_proj(tgt))
         if (small(t->d_tgt, Dl.sa_v, nullptr, t->d_t1, D, D, 0)) return 1;
+        if (stop()) return 0;
         if (small(t->d_t1, Dl.sa_o, t->d_tgt, t->d_t2, D, D, 0)) return 1;
+        if (stop()) return 0;
         if (ln(t->d_t2, Dl.n1, t->d_tgt, B)) return 1;
+        if (stop()) return 0;
         // cross attention: q = W_q (tgt + query_pos)
         add_pos_kernel<<<(B * D / 4 + 255) / 256, 256, 0, st>>>((const float4*)t->d_tgt, (const float4*)t->d_qpos, (float4*)t->d_t1, 1, B, B, D / 4);
         B200_LAUNCH_CHECK();
+        if (stop()) return 0;
         if (small(t->d_t1, Dl.ca_q, nullptr, t->d_q, D, D, 0)) return 1;
+        if (stop()) return 0;
         if (int e = gemm(Dl.g_k)) return e;
+        if (stop()) return 0;
         if (int e = gemm(Dl.g_v)) return e;
+        if (stop()) return 0;
         attention_q1_kernel<<<B * H, 256, (size_t)(L + 8 * AT_HD) * sizeof(float), st>>>(t->d_q, buf(t->b_k), buf(t->b_v), key_padding_mask,
                                                                                          t->d_att, L, B, H, D, D, D, D, scale);
         B200_LAUNCH_CHECK();
+        if (stop()) return 0;
         if (small(t->d_att, Dl.ca_o, t->d_tgt, t->d_t2, D, D, 0)) return 1;
+        if (stop()) return 0;
         if (ln(t->d_t2, Dl.n2, t->d_tgt, B)) return 1;
+        if (stop()) return 0;
         if (small(t->d_tgt, Dl.f1, nullptr, t->d_ff, D, FF, 1)) return 1;
+        if (stop()) return 0;
         if (small(t->d_ff, Dl.f2, t->d_tgt, t->d_t2, FF, D, 0)) return 1;
+        if (stop()) return 0;
         if (ln(t->d_t2, Dl.n3, t->d_tgt, B)) return 1;
+        if (stop()) return 0;
     }
     if (ln(t->d_tgt, t->dec_norm, hs, B)) return 1;
+    return 0;
+}
+
+// ---- debug read-back (tests): stop a forward pass after launch k, copy any internal buffer, report each GEMM's launch plan ----
+namespace b200trk { int tc_conv_grid(const Op& op, int dims[4]); int tc_conv_reduction(const Op& op); int tc_conv_tile(const Op& op, int dims[2]); }
+
+extern "C" int b200trk_transformer_debug_num_launches(const b200trk_transformer_t* t) {
+    return t ? 9 * t->n_enc + 1 + 13 * t->n_dec + 1 : 0;
+}
+
+extern "C" int b200trk_transformer_debug_stop_after(b200trk_transformer_t* t, int launch) {
+    B200_REQUIRE(t && launch >= -1 && launch < b200trk_transformer_debug_num_launches(t), "transformer_debug_stop_after: bad argument");
+    t->stop_after = launch;
+    return 0;
+}
+
+static float* t_debug_buf(const b200trk_transformer_t* t, int id, long long* floats) {
+    const long long BD = (long long)t->B * t->D;
+    if (id >= 0 && id <= 8) { *floats = (long long)t->box.buf_floats[id]; return t->box.bufs[id]; }
+    float* const dec[7] = {t->d_tgt, t->d_t1, t->d_t2, t->d_q, t->d_att, t->d_ff, t->d_qpos};
+    if (id >= 9 && id <= 15) { *floats = id == 14 ? (long long)t->B * t->FF : BD; return dec[id - 9]; }
+    return nullptr;
+}
+
+extern "C" int b200trk_transformer_debug_buffer(const b200trk_transformer_t* t, int buf, float* dst, long long* floats, b200trk_stream_t stream) {
+    long long n = 0;
+    float* p = t ? t_debug_buf(t, buf, &n) : nullptr;
+    B200_REQUIRE(p, "transformer_debug_buffer: bad argument (buffer id %d)", buf);
+    if (floats) *floats = n;
+    if (dst) B200_CHECK_CUDA(cudaMemcpyAsync(dst, p, (size_t)n * sizeof(float), cudaMemcpyDeviceToDevice, (cudaStream_t)stream));
+    return 0;
+}
+
+extern "C" int b200trk_transformer_debug_gemm(const b200trk_transformer_t* t, int gemm, int info[15]) {
+    B200_REQUIRE(t && info && gemm >= 0 && gemm < (int)t->gemms.size(), "transformer_debug_gemm: bad argument");
+    const Op& op = t->gemms[gemm];
+    int g[4], tile[2];
+    tc_conv_grid(op, g);
+    tc_conv_tile(op, tile);
+    const int v[15] = {op.in, op.out, op.res, op.relu, op.Hin, op.Win, op.Cin, op.Cout, g[0], g[1], g[2], g[3], tc_conv_reduction(op), tile[0],
+                       tile[1]};
+    memcpy(info, v, sizeof(v));
     return 0;
 }
