@@ -1,4 +1,6 @@
-"""TEST INFRASTRUCTURE ONLY -- CPU restatement (torch-CPU fp32) of the ATOM rows of the hot path.
+"""TEST INFRASTRUCTURE ONLY -- CPU restatement (torch-CPU) of the ATOM rows of the hot path.  Every function computes in the dtype
+of its inputs: float32 inputs give the float32 restatement the goldens pin, float64 inputs a float64 computation throughout (the
+sums that are accumulated in float64 are rounded back to the input dtype, never to float32).
 
 Same rules as oracle/dimp_oracle.py: only tests/, __graft_entry__.smoke() and bench.py's CPU legs may import it.
 Parity status: PINNED -- `oracle/gen_golden.py` (gen_atom_cg, gen_fourier) runs the unmodified reference classes
@@ -34,7 +36,7 @@ def conv_same_adjoint_filter(x, u, k):
     xp = F.pad(x, (p, p, p, p))
     win = xp.unfold(2, k, 1).unfold(3, k, 1)                 # [n,c,H+1,W+1,k,k] for even k
     win = win[:, :, :u.shape[-2], :u.shape[-1]]
-    return torch.einsum("ncyxab,nyx->cab", win.double(), u[:, 0].double()).float().unsqueeze(0)
+    return torch.einsum("ncyxab,nyx->cab", win.double(), u[:, 0].double()).to(x.dtype).unsqueeze(0)
 
 
 def conv1x1(x, P):
@@ -59,7 +61,7 @@ def activation_deriv(x, kind="none", param=0.05):
     if kind == "none":
         return torch.ones_like(x)
     if kind == "relu":
-        return (x > 0).float()
+        return (x > 0).to(x.dtype)
     if kind == "elu":
         return torch.where(x > 0, torch.ones_like(x), torch.exp(x))
     if kind == "mlu":
@@ -70,13 +72,16 @@ def activation_deriv(x, kind="none", param=0.05):
 # ----------------------------------------------------------------------------------------------
 # S3.5 ConjugateGradient.run on ConvProblem (the per-frame ATOM filter update)
 # ----------------------------------------------------------------------------------------------
-def atom_cg_filter(w, feat, y, sw, filter_reg, num_iter, act="mlu", act_param=0.05, fletcher_reeves=False):
+def atom_cg_filter(w, feat, y, sw, filter_reg, num_iter, act="mlu", act_param=0.05, fletcher_reeves=False, dact=None):
     """ConjugateGradient.run(num_iter) (pytracking/libs/optimization.py:227-275, run_CG :72-163) on
     ConvProblem (pytracking/tracker/atom/optim.py:71-99), direction_forget_factor = 0 (state reset every run).
-    w [1,C,k,k], feat [n,C,H,W], y [n,1,H,W], sw [n]. Returns (w_new, delta, rho_trace)."""
+    w [1,C,k,k], feat [n,C,H,W], y [n,1,H,W], sw [n]; dact [n,1,H,W] replaces phi'(s) when given (the tests take the
+    derivative of a cell at a kink from its other side with it). Returns (w_new, delta, rho_trace)."""
     k = w.shape[-1]
     s = conv_same(feat, w)
     a, d = activation(s, act, act_param), activation_deriv(s, act, act_param)
+    if dact is not None:
+        d = dact
     swv = sw.view(-1, 1, 1, 1)
     # b = -J^T f0,  f0 = [sqrt(sw) (phi(s) - y), sqrt(reg) w],  J^T u = A^T(sqrt(sw) phi' u_data) + sqrt(reg) u_reg
     b = -(conv_same_adjoint_filter(feat, swv * d * (a - y), k) + filter_reg * w)
@@ -86,7 +91,7 @@ def atom_cg_filter(w, feat, y, sw, filter_reg, num_iter, act="mlu", act_param=0.
         return conv_same_adjoint_filter(feat, D * conv_same(feat, p), k) + filter_reg * p
 
     def ip(u, v):
-        return (u.double() * v.double()).sum().float()
+        return (u.double() * v.double()).sum().to(u.dtype)
 
     r = b.clone()
     x = None
@@ -151,7 +156,7 @@ def fourier_interp(scores, kernel_size, output_sz):
     mid = int((f.shape[2] - 1) / 2)
     f = torch.cat((f[:, :, mid:, :], f[:, :, :mid, :]), 2)                    # irfftshift2
     out = torch.fft.irfftn(f, s=(oh, ow), dim=(-2, -1)) * (oh * ow)
-    return out.float()
+    return out.to(scores.dtype)
 
 
 def feature_normalize(x, p=2.0):
@@ -181,7 +186,7 @@ def atom_gn_joint(w, P, X, y, sw, filter_reg, proj_reg, num_cg_iter, num_gn_iter
     w, P = w.clone(), P.clone()
 
     def ip(a, b):
-        return (a[0].double() * b[0].double()).sum().float() + (a[1].double() * b[1].double()).sum().float()
+        return (a[0].double() * b[0].double()).sum().to(a[0].dtype) + (a[1].double() * b[1].double()).sum().to(a[1].dtype)
 
     for _ in range(num_gn_iter):
         comp = conv1x1(X, P)
@@ -193,7 +198,7 @@ def atom_gn_joint(w, P, X, y, sw, filter_reg, proj_reg, num_cg_iter, num_gn_iter
         def JT(u):      # u already carries sw * phi' factors
             gw = conv_same_adjoint_filter(comp, u, k)
             T = conv_same_adjoint_input(u, w, H, Wd)                  # [n,Cc,H,W]
-            gP = torch.einsum("ncp,nkp->ck", T.flatten(2).double(), X.flatten(2).double()).float().reshape(P.shape)
+            gP = torch.einsum("ncp,nkp->ck", T.flatten(2).double(), X.flatten(2).double()).to(X.dtype).reshape(P.shape)
             return gw, gP
 
         gw, gP = JT(r0)

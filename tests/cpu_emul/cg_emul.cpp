@@ -2,12 +2,24 @@
 // cooperative kernel on the cp.async sweeps of csrc/corr2.cuh -- the same sources the CUDA build compiles) on the CPU under cuda_shim.h.
 // Two builds: plain (OS thread per CUDA thread, what ThreadSanitizer needs) runs ONE CTA -- the kernel keeps small arrays in static __shared__
 // storage, which that mode can give to a single live block only; with -DB200_EMUL_COOP_FIBERS (a block = one OS thread, its threads = fibers,
-// static __shared__ = thread_local) the grid is the one launch_cg (csrc/atom_cg.cu) picks for `sms` SMs, cross-CTA exchange included.  Built and called by tests/test_sd_kernels_cpu.py.
+// static __shared__ = thread_local) the grid is the one launch_cg (csrc/atom_cg.cu) picks for `sms` SMs, cross-CTA exchange included.  The pipeline depth NST
+// is the one launch_cg picks (4, 3 or 2 stages).  Built and called by tests/test_sd_kernels_cpu.py and tests/test_atom_step_ref_cpu.py.
 #include "cuda_shim.h"
 
 #include "../../pytracking_b200/csrc/atom_cg_kernel.cuh"
 
 using namespace b200trk;
+
+template <int FS, int NST>
+static int launch_nst(const CgParams& P, int ctas, size_t smem) {
+#ifdef B200_EMUL_COOP_FIBERS
+    cpu_emul::launch_coop(atom_cg_kernel<FS, NST>, (unsigned)ctas, (unsigned)Corr2<FS>::NCONS, smem, P);
+#else
+    (void)ctas;
+    cpu_emul::launch(atom_cg_kernel<FS, NST>, 1u, (unsigned)Corr2<FS>::NCONS, smem, P);
+#endif
+    return 0;
+}
 
 template <int FS>
 static int run_cg(CgParams P, int sms) {
@@ -35,12 +47,12 @@ static int run_cg(CgParams P, int sms) {
     const int cchunk = passes * K::SLOTS;
     const size_t fixed = (size_t)(K::NT * K::SLOTS * K::RED_STRIDE + 6 * cchunk * K::VEC_STRIDE + spc * (2 * K::NPOS + K::PMAP) + K::NCONS * 4) * sizeof(float);
     const size_t item = (size_t)K::ITEM_FLOATS * sizeof(float);
-#ifdef B200_EMUL_COOP_FIBERS
-    cpu_emul::launch_coop(atom_cg_kernel<FS, 2>, (unsigned)(NCH * NG), (unsigned)K::NCONS, fixed + 2 * item, P);
-#else
-    cpu_emul::launch(atom_cg_kernel<FS, 2>, 1u, (unsigned)K::NCONS, fixed + 2 * item, P);
-#endif
-    return 0;
+    // pipeline depth as launch_cg picks it from the shared-memory budget (227 KB less the static arrays)
+    const size_t limit = 227 * 1024 - 512;
+    if (fixed + 4 * item <= limit) return launch_nst<FS, 4>(P, NCH * NG, fixed + 4 * item);
+    if (fixed + 3 * item <= limit) return launch_nst<FS, 3>(P, NCH * NG, fixed + 3 * item);
+    if (fixed + 2 * item > limit) return 2;
+    return launch_nst<FS, 2>(P, NCH * NG, fixed + 2 * item);
 }
 
 extern "C" int cg_emul_atom_cg_filter(const float* filter, float* filter_out, const float* feat, const float* y, const float* sample_weight, int n, int C,
