@@ -654,28 +654,59 @@ __global__ void __launch_bounds__(STC_THREADS, 1) sd_tc_kernel(const __grid_cons
         SD_STAMP(tb + 3);
 
         // ---- this CTA's slice of g = sum of the partial gradients + reg * w --------------------------------------------------------
+        // Warp w sums entries sl_lo + w, + 9, ... ; lane l adds the partials of contributors bf + l, + 32, ... in that order. The
+        // loads of two entries and of up to SL_GB contributors per lane are issued before the first add, so a warp waits for L2
+        // once per pass instead of once per contributor batch and entry; the order of every sum is the one written above.
         float gl = 0.f;
         {
+            constexpr int SL_GB = 4;
             const int per_chunk = n * KBT;
-            for (int e = sl_lo + warp; e < sl_hi; e += NTH / 32) {
-                const int chunk = e >> 9, within = e & 511;                   // 128 channels x 16 taps = 512 float4 per chunk
-                const int bf = s_bf[chunk], bl = s_bl[chunk];
-                float4 a = make_float4(0.f, 0.f, 0.f, 0.f);
-                for (int bb = bf + lane; bb <= bl; bb += 32) {
-                    const int lo = s_tlo[bb], hi = s_tlo[bb + 1];
-                    if (hi > lo) {
-                        const int cl = chunk - lo / per_chunk;
-                        const float4 v = __ldcg(reinterpret_cast<const float4*>(Q.gpart) + ((size_t)bb * STC_MAXCH + cl) * 512 + within);
-                        a.x += v.x; a.y += v.y; a.z += v.z; a.w += v.w;
-                    }
+            for (int e0 = sl_lo + warp; e0 < sl_hi; e0 += 2 * (NTH / 32)) {
+                float4 a[2];
+                int bf[2], bl[2];
+#pragma unroll
+                for (int q = 0; q < 2; ++q) {
+                    const int e = e0 + q * (NTH / 32), chunk = e >> 9;       // 128 channels x 16 taps = 512 float4 per chunk
+                    a[q] = make_float4(0.f, 0.f, 0.f, 0.f);
+                    bf[q] = (e < sl_hi) ? s_bf[chunk] : 0;
+                    bl[q] = (e < sl_hi) ? s_bl[chunk] : -1;
                 }
-                a.x = warp_sum_xor(a.x); a.y = warp_sum_xor(a.y); a.z = warp_sum_xor(a.z); a.w = warp_sum_xor(a.w);
-                if (lane == 0) {
-                    const float4 w = wsl[e - sl_lo];
-                    a.x += reg * w.x; a.y += reg * w.y; a.z += reg * w.z; a.w += reg * w.w;
-                    gsl[e - sl_lo] = a;
-                    __stcg(reinterpret_cast<float4*>(Q.gfinal) + e, a);
-                    gl += a.x * a.x + a.y * a.y + a.z * a.z + a.w * a.w;
+                const int span = max(bl[0] - bf[0], bl[1] - bf[1]) + 1;
+                for (int k0 = 0; k0 < span; k0 += 32 * SL_GB) {
+                    float4 v[2][SL_GB];
+                    bool ok[2][SL_GB];
+#pragma unroll
+                    for (int q = 0; q < 2; ++q)
+#pragma unroll
+                        for (int k = 0; k < SL_GB; ++k) {
+                            const int e = e0 + q * (NTH / 32), chunk = e >> 9, within = e & 511;
+                            const int bb = bf[q] + k0 + lane + 32 * k;
+                            int lo = 0;
+                            ok[q][k] = false;
+                            if (bb <= bl[q]) { lo = s_tlo[bb]; ok[q][k] = s_tlo[bb + 1] > lo; }
+                            v[q][k] = ok[q][k] ? __ldcg(reinterpret_cast<const float4*>(Q.gpart) +
+                                                        ((size_t)bb * STC_MAXCH + (chunk - lo / per_chunk)) * 512 + within)
+                                               : make_float4(0.f, 0.f, 0.f, 0.f);
+                        }
+#pragma unroll
+                    for (int q = 0; q < 2; ++q)
+#pragma unroll
+                        for (int k = 0; k < SL_GB; ++k)
+                            if (ok[q][k]) { a[q].x += v[q][k].x; a[q].y += v[q][k].y; a[q].z += v[q][k].z; a[q].w += v[q][k].w; }
+                }
+#pragma unroll
+                for (int q = 0; q < 2; ++q) {
+                    const int e = e0 + q * (NTH / 32);
+                    if (e >= sl_hi) break;                                    // (warp-uniform)
+                    float4 s = a[q];
+                    s.x = warp_sum_xor(s.x); s.y = warp_sum_xor(s.y); s.z = warp_sum_xor(s.z); s.w = warp_sum_xor(s.w);
+                    if (lane == 0) {
+                        const float4 w = wsl[e - sl_lo];
+                        s.x += reg * w.x; s.y += reg * w.y; s.z += reg * w.z; s.w += reg * w.w;
+                        gsl[e - sl_lo] = s;
+                        __stcg(reinterpret_cast<float4*>(Q.gfinal) + e, s);
+                        gl += s.x * s.x + s.y * s.y + s.z * s.z + s.w * s.w;
+                    }
                 }
             }
         }
@@ -732,8 +763,19 @@ __global__ void __launch_bounds__(STC_THREADS, 1) sd_tc_kernel(const __grid_cons
 
         // ---- step length and update ------------------------------------------------------------------------------------------------
         if (warp == 0) {
+            // lane l sums the partials of CTAs l, l + 32, ... in that order, all loads in flight before the first add
+            constexpr int GL = (STC_MAXG + 31) / 32;
+            float vg[GL], vh[GL];
+#pragma unroll
+            for (int t = 0; t < GL; ++t) {
+                const int k = lane + 32 * t;
+                vg[t] = (k < G) ? __ldcg(Q.gnpart + k) : 0.f;
+                vh[t] = (k < G) ? __ldcg(Q.hpart + k) : 0.f;
+            }
             float gn = 0.f, hn = 0.f;
-            for (int k = lane; k < G; k += 32) { gn += __ldcg(Q.gnpart + k); hn += __ldcg(Q.hpart + k); }
+#pragma unroll
+            for (int t = 0; t < GL; ++t)
+                if (lane + 32 * t < G) { gn += vg[t]; hn += vh[t]; }
             gn = warp_sum_xor(gn); hn = warp_sum_xor(hn);
             if (lane == 0) {
                 const float den = fmaxf(hn + (reg + P.alpha_eps) * gn, 1e-8f);
