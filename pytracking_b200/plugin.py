@@ -18,7 +18,7 @@ import weakref
 
 import torch
 
-from . import ops
+from . import eco_plan, ops
 from .engine import BackboneEngine
 from .iou import IoUPredictor
 from .transformer_engine import BoxTower, TokenBuilder, TransformerEngine
@@ -474,7 +474,7 @@ def _eco_gn_run(self, num_cg_iter, num_gn_iter=None):
                 rf.dim() == 4 and rf.shape[-2] <= min(8, hf.shape[2]) and rf.shape[-1] <= min(8, hf.shape[3]) and \
                 p.sample_weights_sqrt[b].numel() in (1, xs.shape[2]) and p.diag_M[b].numel() == hf.numel() // 2 and \
                 xs.shape[2] <= 1024 and pm.shape[0] <= 4096 and hf.shape[1] <= 512 and float(p.diag_M[nblk + b]) > 0 and \
-                4 * (980 + 17 * ((xs.shape[2] + 3) & ~3) + 8 * (4 * hf.shape[1] + 2 * pm.shape[0])) <= 226 * 1024   # ecoj_fixed_smem_floats
+                eco_plan.eco_joint_fits(xs.shape[2], pm.shape[0], hf.shape[1])
     if not ok:
         raise NotImplementedError("b200trk GaussNewtonCG.run: ECO feature blocks the joint kernel does not take")
     for b in range(nblk):

@@ -334,10 +334,11 @@ def test_joint_seam_over_the_emulated_kernel(emul, jgold, monkeypatch):
 
 def test_joint_launch_plan_at_eco_block_sizes(emul):
     """ECO default first frame: 30 augmented samples; deep block 256 -> 64 channels on ~15x8 coefficients, shallow 96 -> 16 on ~63x32."""
-    # the shared-memory arithmetic of eco_joint_plan, through the Python mirror the plug-in guard uses (plugin.py, gn_run)
+    # the shared-memory arithmetic of eco_joint_plan, through the Python mirror the plug-in guard uses (pytracking_b200/eco_plan.py)
+    from pytracking_b200 import eco_plan
     for n, cin, c in ((30, 256, 64), (30, 96, 16), (30, 512, 128)):
-        n4 = (n + 3) & ~3
-        fixed = 4 * (980 + 17 * n4 + 8 * (4 * c + 2 * cin))
+        fixed = 4 * eco_plan.ecoj_fixed_smem_floats(n, cin, c)
+        assert eco_plan.eco_joint_fits(n, cin, c)
         slab = n * (cin + 1) * 8
         assert fixed <= 226 * 1024
         assert (227 * 1024 - 1024 - fixed) // slab >= 1                # at least one coefficient's slab resident per CTA
