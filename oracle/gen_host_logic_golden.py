@@ -1,7 +1,7 @@
 """TEST INFRASTRUCTURE ONLY -- records what the host half of the native whole-frame tracker (csrc/dimp_tracker.cu: plan_crop / commit)
 and its two small kernels (sample_patch, localize) must reproduce, from the UNMODIFIED reference DiMP tracker run on the CPU.
 
-    python -m oracle.gen_host_logic_golden [cfg2|stress|noaug|localize]      (needs a reference checkout: baseline/_ref or PYTRACKING_REFERENCE)
+    python -m oracle.gen_host_logic_golden [cfg2|stress|noaug|localize|localize_nan]      (needs a reference checkout: baseline/_ref or PYTRACKING_REFERENCE)
 
 Per configuration (`tests/golden/dimp_host_<name>.npz`): the scalar state after DiMP.initialize, and per frame the crop request
 (sample_patch's patch_coord), the score map, both dcf.max2d results and the flag of localize_advanced, the output box, the memory
@@ -11,7 +11,8 @@ update (slot, target box, learning rate, sample weights) and the optimiser itera
              (not_found / uncertain / hard_negative by either maximum / normal), memory wrap-around and train_skipping > 1 occur
   noaug   -- use_augmentation=False, filter_init_zero=True: the configuration the native initialisation implements
 and `tests/golden/dimp_localize_random.npz`: the reference's `DiMP.localize_target` (translation, scale index, flag) on the 400 seeded
-problems of tests/tracker_cases.py:random_localize_cases.
+problems of tests/tracker_cases.py:random_localize_cases, and `tests/golden/dimp_localize_nan.npz` (target localize_nan): the same on
+the NaN maps of tests/tracker_cases.py:nan_localize_cases.
 """
 import os
 import sys
@@ -177,6 +178,37 @@ def record_localize():
                         scale_ind=np.array(scale_ind), flag=np.array(flag))
 
 
+def record_localize_nan():
+    import types
+    from oracle import ref_shims
+    ref_shims.install(prroi_cpu=False)
+    from pytracking.tracker.dimp.dimp import DiMP
+    from pytracking.utils import TrackerParams
+    sys.path.insert(0, os.path.join(ROOT, "tests"))
+    from tracker_cases import nan_localize_cases
+    tv, scale_ind, flag = [], [], []
+    for trial, kw, reg, scores, target_sz, sample_scales, sample_pos, pos in nan_localize_cases():
+        trk = DiMP.__new__(DiMP)
+        p = TrackerParams()
+        for k, v in kw.items():
+            setattr(p, k, v)
+        p.target_neighborhood_scale = 2.2
+        trk.params = p
+        trk.net = types.SimpleNamespace(classifier=types.SimpleNamespace(filter_optimizer=types.SimpleNamespace(softmax_reg=reg)))
+        trk.output_window = None
+        trk.kernel_size = torch.Tensor([4, 4])
+        trk.img_support_sz = torch.Tensor([288, 288])
+        trk.target_sz = target_sz
+        trk.pos = pos
+        t, si, _, f = trk.localize_target(scores.clone().unsqueeze(1), sample_pos, sample_scales)
+        tv.append(t.numpy())
+        scale_ind.append(int(si))
+        flag.append(FLAG[f])
+    np.savez_compressed(os.path.join(GOLDEN, "dimp_localize_nan.npz"), translation=np.array(tv, dtype=np.float32),
+                        scale_ind=np.array(scale_ind), flag=np.array(flag))
+
+
 if __name__ == "__main__":
-    for name in (sys.argv[1:] or list(CONFIGS) + ["localize"]):
-        record_localize() if name == "localize" else record(name, CONFIGS[name])
+    targets = {"localize": record_localize, "localize_nan": record_localize_nan}
+    for name in (sys.argv[1:] or list(CONFIGS) + list(targets)):
+        targets[name]() if name in targets else record(name, CONFIGS[name])

@@ -242,11 +242,14 @@ template <int FS> struct CorrSlots;
 template <> struct CorrSlots<18> { static constexpr int value = 16; };
 template <> struct CorrSlots<22> { static constexpr int value = 8; };
 
-// Reference arg-max order (pytracking/libs/dcf.py:156-164): larger value; ties -> smaller column, then smaller row.
+// Reference arg-max order (pytracking/libs/dcf.py:156-164): larger value; ties -> smaller column, then smaller row.  torch.max
+// propagates NaN, so NaN ranks above every value and all NaNs tie: a map holding NaN reports its first NaN in the tie order.
 struct ArgMax {
     float v; int row, col;
     __device__ __forceinline__ bool better_than(const ArgMax& o) const {
-        if (v != o.v) return v > o.v;
+        const bool nan = v != v, onan = o.v != o.v;
+        if (nan != onan) return nan;
+        if (!nan && v != o.v) return v > o.v;
         if (col != o.col) return col < o.col;
         return row < o.row;
     }

@@ -5,22 +5,15 @@
 
 namespace b200trk {
 
-static int pick_passes(int C, int slots, int max_passes) {
-    for (int p = max_passes; p >= 1; p >>= 1)
-        if (C % (slots * p) == 0) return p;
-    return 0;
-}
-
 template <int FS>
 static int launch_apply_filter(const float* feat, const float* filt, float* scores, int n, int C,
                                float* max_val, int64_t* max_idx, cudaStream_t st, int crop = 0) {
     constexpr int SLOTS = CorrSlots<FS>::value;
     using K = CorrCta<FS, SLOTS>;
     using G = CorrGeom<FS>;
-    // few samples at classification time (S scales): spread channels over many CTAs
-    int passes = pick_passes(C, SLOTS, n >= 16 ? 4 : 1);
+    const CorrPlan plan = corr_plan(0, n, C, SLOTS, 0);
+    const int passes = plan.passes, NCH = plan.nch;
     B200_REQUIRE(passes > 0, "apply_filter: C=%d must be a multiple of %d for feature size %d", C, SLOTS, FS);
-    const int NCH = C / (SLOTS * passes);
     B200_REQUIRE(n <= 1024, "apply_filter: n=%d > 1024 maps per call", n);
     // workspace layout: [0,4096) per-sample arrival counters (zero at allocation, self-resetting), then partial maps
     const size_t part_bytes = (size_t)n * NCH * G::NPOS * sizeof(float);
@@ -41,14 +34,9 @@ static int launch_feat_transpose(const float* feat, const float* resid, float* g
     constexpr int SLOTS = CorrSlots<FS>::value;
     using K = CorrCta<FS, SLOTS>;
     using G = CorrGeom<FS>;
-    int passes = pick_passes(C, SLOTS, 4);
+    const CorrPlan plan = corr_plan(1, n, C, SLOTS, device_sm_count());
+    const int passes = plan.passes, NCH = plan.nch, NG = plan.ng, spc_max = plan.spc_max;
     B200_REQUIRE(passes > 0, "apply_feat_transpose: C=%d must be a multiple of %d for feature size %d", C, SLOTS, FS);
-    const int NCH = C / (SLOTS * passes);
-    const int sms = device_sm_count();
-    int NG = sms / NCH; if (NG < 1) NG = 1; if (NG > n) NG = n;
-    const int SPC_CAP = 8;
-    if ((n + NG - 1) / NG > SPC_CAP) NG = (n + SPC_CAP - 1) / SPC_CAP;
-    const int spc_max = (n + NG - 1) / NG;
     B200_REQUIRE(NCH <= 1024, "apply_feat_transpose: too many channel chunks (%d)", NCH);
     const size_t gp_bytes = (size_t)NG * C * 16 * sizeof(float);
     char* ws = (char*)workspace(4096 + gp_bytes, 1);

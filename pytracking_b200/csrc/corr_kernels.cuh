@@ -15,6 +15,33 @@
 namespace b200trk {
 
 // --------------------------------------------------------------------------------------------------
+// Launch plan of apply_filter_kernel (transpose = 0, grid (nch, n)) and feat_transpose_kernel (transpose = 1, grid (nch, ng)) for n
+// samples of C channels with `slots` planes per CTA on a device of `sms` SMs.  Host code, shared by corr_api.cu and the CPU tier
+// (tests/cpu_emul/corr_emul.cpp).  passes = 0 when C is not a multiple of `slots`.
+// --------------------------------------------------------------------------------------------------
+struct CorrPlan {
+    int passes;    // channel planes each slot sweeps per sample: 4, 2 or 1 (apply: 1 below 16 samples, to spread C over many CTAs)
+    int nch;       // channel chunks of passes * slots channels
+    int ng;        // sample groups (apply: n, one sample each)
+    int spc_max;   // samples of the largest group (apply: 1)
+};
+
+inline CorrPlan corr_plan(int transpose, int n, int C, int slots, int sms) {
+    CorrPlan p{0, 0, n, 1};
+    for (int q = (transpose || n >= 16) ? 4 : 1; q >= 1 && !p.passes; q >>= 1)
+        if (C % (slots * q) == 0) p.passes = q;
+    if (!p.passes) return p;
+    p.nch = C / (slots * p.passes);
+    if (!transpose) return p;
+    int NG = sms / p.nch; if (NG < 1) NG = 1; if (NG > n) NG = n;
+    const int SPC_CAP = 8;                                   // residual planes staged in shared memory per CTA
+    if ((n + NG - 1) / NG > SPC_CAP) NG = (n + SPC_CAP - 1) / SPC_CAP;
+    p.ng = NG;
+    p.spc_max = (n + NG - 1) / NG;
+    return p;
+}
+
+// --------------------------------------------------------------------------------------------------
 // max2d over [n,H,W] maps: one CTA per map. Also used as the tail of apply_filter.
 // --------------------------------------------------------------------------------------------------
 __device__ __forceinline__ ArgMax argmax_block(const float* a, int H, int W, ArgMax* sred) {

@@ -96,9 +96,12 @@ struct LocArgs {
 };
 
 struct AM { float v; int r, c; };
-// dcf.max2d order (pytracking/libs/dcf.py:156-164): the column of the maximum first (smallest on ties), then the smallest row
+// dcf.max2d order (pytracking/libs/dcf.py:156-164): the column of the maximum first (smallest on ties), then the smallest row; NaN
+// above every value and all NaNs tied, as torch.max propagates NaN (ArgMax::better_than, corr.cuh)
 __device__ __forceinline__ bool am_better(const AM& a, const AM& b) {
-    if (a.v != b.v) return a.v > b.v;
+    const bool an = a.v != a.v, bn = b.v != b.v;
+    if (an != bn) return an;
+    if (!an && a.v != b.v) return a.v > b.v;
     if (a.c != b.c) return a.c < b.c;
     return a.r < b.r;
 }
@@ -183,7 +186,8 @@ __device__ __forceinline__ void localize_body(const float* __restrict__ scores_i
         __syncthreads();
         scores = pre;
     }
-    // max_score1, max_disp1 per scale; scale_ind = first scale with the largest maximum (torch.max(max_score1, dim=0))
+    // max_score1, max_disp1 per scale; scale_ind = first scale with the largest maximum (torch.max(max_score1, dim=0)), the first
+    // NaN maximum if there is one
     AM best1 = none; int scale_ind = 0;
     for (int s = 0; s < a.S; ++s) {
         AM m = none;
@@ -192,7 +196,7 @@ __device__ __forceinline__ void localize_body(const float* __restrict__ scores_i
             if (am_better(t, m)) m = t;
         }
         m = block_argmax(m, red);
-        if (s == 0 || m.v > best1.v) { best1 = m; scale_ind = s; }
+        if (s == 0 || m.v > best1.v || (m.v != m.v && best1.v == best1.v)) { best1 = m; scale_ind = s; }
     }
     b200trk_loc_result_t out;
     out.flag = 0; out.scale_ind = scale_ind; out.r1 = best1.r; out.c1 = best1.c; out.r2 = -1; out.c2 = -1; out.use_second = 0;

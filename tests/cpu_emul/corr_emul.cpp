@@ -1,27 +1,22 @@
 // TEST INFRASTRUCTURE ONLY.  Runs csrc/corr_kernels.cuh (+ corr.cuh: dcf.max2d, apply_filter with the fused arg-max / 'same' crop,
-// apply_feat_transpose -- the same source the CUDA build compiles) on the CPU under cuda_shim.h with the launch arithmetic of
-// csrc/corr_api.cu (channel chunks, sample groups, the self-resetting arrival counters).  Built and called by tests/test_corr_kernels_cpu.py.
+// apply_feat_transpose -- the same source the CUDA build compiles) on the CPU under cuda_shim.h with the launch plan csrc/corr_api.cu
+// launches with (corr_plan: channel chunks, sample groups) and the self-resetting arrival counters, kept across calls as in the library's
+// workspace.  Built and called by tests/test_corr_kernels_cpu.py and tests/test_corr_f64_cpu.py.
 #include "cuda_shim.h"
 
 #include "../../pytracking_b200/csrc/corr_kernels.cuh"
 
 using namespace b200trk;
 
-static int pick_passes(int C, int slots, int max_passes) {
-    for (int p = max_passes; p >= 1; p >>= 1)
-        if (C % (slots * p) == 0) return p;
-    return 0;
-}
-
 template <int FS>
 static int run_apply(const float* feat, const float* filt, float* scores, int n, int C, float* max_val, int64_t* max_idx, int crop) {
     constexpr int SLOTS = CorrSlots<FS>::value;
     using K = CorrCta<FS, SLOTS>;
     using G = CorrGeom<FS>;
-    const int passes = pick_passes(C, SLOTS, n >= 16 ? 4 : 1);
+    const CorrPlan plan = corr_plan(0, n, C, SLOTS, 0);
+    const int passes = plan.passes, NCH = plan.nch;
     if (passes <= 0) return 2;
-    const int NCH = C / (SLOTS * passes);
-    std::vector<unsigned> counters(1024, 0u);
+    static std::vector<unsigned> counters(1024, 0u);
     std::vector<float> part((size_t)n * NCH * G::NPOS, -1e30f);
     const size_t smem = (size_t)(K::PLANES_FLOATS + K::RED_FLOATS + passes * SLOTS * 16) * sizeof(float);
     cpu_emul::launch_blocks(apply_filter_kernel<FS, SLOTS>, (unsigned)NCH, (unsigned)n, 1u, (unsigned)K::NTHREADS, smem, feat, filt, scores, part.data(),
@@ -35,14 +30,10 @@ static int run_transpose(const float* feat, const float* resid, float* grad, int
     constexpr int SLOTS = CorrSlots<FS>::value;
     using K = CorrCta<FS, SLOTS>;
     using G = CorrGeom<FS>;
-    const int passes = pick_passes(C, SLOTS, 4);
+    const CorrPlan plan = corr_plan(1, n, C, SLOTS, sms);
+    const int passes = plan.passes, NCH = plan.nch, NG = plan.ng, spc_max = plan.spc_max;
     if (passes <= 0) return 2;
-    const int NCH = C / (SLOTS * passes);
-    int NG = sms / NCH; if (NG < 1) NG = 1; if (NG > n) NG = n;
-    const int SPC_CAP = 8;
-    if ((n + NG - 1) / NG > SPC_CAP) NG = (n + SPC_CAP - 1) / SPC_CAP;
-    const int spc_max = (n + NG - 1) / NG;
-    std::vector<unsigned> counters(1024, 0u);
+    static std::vector<unsigned> counters(1024, 0u);
     std::vector<float> gpart((size_t)NG * C * 16, -1e30f);
     const size_t smem = (size_t)(K::PLANES_FLOATS + K::RED_FLOATS + spc_max * G::NPOS) * sizeof(float);
     cpu_emul::launch_blocks(feat_transpose_kernel<FS, SLOTS>, (unsigned)NCH, (unsigned)NG, 1u, (unsigned)K::NTHREADS, smem, feat, resid, grad, gpart.data(),
@@ -62,6 +53,15 @@ extern "C" int corr_emul_feat_transpose(const float* feat, const float* resid, f
     if (H == 18 && W == 18) return run_transpose<18>(feat, resid, grad, n, C, sms);
     if (H == 22 && W == 22) return run_transpose<22>(feat, resid, grad, n, C, sms);
     return 2;
+}
+
+// corr_plan of corr_kernels.cuh for feature size FS: out = {passes, nch, ng, spc_max, slots}
+extern "C" int corr_emul_plan(int transpose, int n, int C, int FS, int sms, int* out) {
+    const int slots = FS == 18 ? CorrSlots<18>::value : FS == 22 ? CorrSlots<22>::value : 0;
+    if (!slots) return 2;
+    const CorrPlan p = corr_plan(transpose, n, C, slots, sms);
+    out[0] = p.passes; out[1] = p.nch; out[2] = p.ng; out[3] = p.spc_max; out[4] = slots;
+    return 0;
 }
 
 extern "C" int corr_emul_max2d(const float* a, int n, int H, int W, float* max_val, int64_t* max_idx) {

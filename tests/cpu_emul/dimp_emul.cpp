@@ -16,6 +16,6 @@ extern "C" int dimp_emul_localize(const float* scores, int S, int Ho, int Wo, co
                                   const float* prev_vec, b200trk_loc_result_t* result) {
     if (S < 1 || S > 8) return 2;
     const LocArgs a = make_loc_args(S, Ho, Wo, p, neigh, prev_vec);
-    cpu_emul::launch_blocks(localize_kernel, 1u, 1u, 1u, 256u, (size_t)0, scores, a, result);    // b200trk_dimp_localize: one CTA of 256 threads
+    cpu_emul::launch_blocks(localize_kernel, 1u, 1u, 1u, 256u, loc_smem_bytes(a), scores, a, result);    // b200trk_dimp_localize: one CTA of 256 threads
     return 0;
 }

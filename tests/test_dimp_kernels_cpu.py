@@ -125,3 +125,25 @@ def test_localize_kernel_source_matches_reference_code_on_random_maps(emul):
         assert torch.equal(mine, torch.from_numpy(gold["translation"][trial])), (trial, mine, gold["translation"][trial])
         seen.add((flag, out.use_second))
     assert {("normal", 0), ("hard_negative", 0), ("hard_negative", 1), ("uncertain", 0), ("not_found", 0), (None, 0)} <= seen, seen
+
+
+def test_localize_kernel_source_matches_reference_code_on_nan_maps(emul):
+    """NaN in the score maps (tests/tracker_cases.py:nan_localize_cases: one NaN cell inside and outside the target neighbourhood, a NaN
+    column, a NaN scale, an all-NaN map; no pre-processing, 'exp' and 'softmax'): flag, scale index and translation exactly as the
+    reference's `localize_target` gives them (tests/golden/dimp_localize_nan.npz).  torch.max propagates NaN, so the reference picks the
+    first NaN cell and the first NaN scale."""
+    from tracker_cases import nan_localize_cases
+    from pytracking_b200.tracker import FLAGS
+    gold = np.load(os.path.join(GOLDEN, "dimp_localize_nan.npz"))
+    code = {None: 0, "normal": 1, "hard_negative": 2, "uncertain": 3, "not_found": 4}
+    img_support_sz, out_sz = torch.Tensor([288, 288]), torch.Tensor([18, 18])
+    for trial, kw, reg, scores, target_sz, sample_scales, sample_pos, pos in nan_localize_cases():
+        S = scores.shape[0]
+        neigh = [(2.2 * (target_sz / sample_scales[s]) * (out_sz / img_support_sz)).numpy() for s in range(S)]
+        pv = [((pos - sample_pos[s]) / ((img_support_sz / out_sz) * sample_scales[s])).numpy() for s in range(S)]
+        out = _run_localize(emul, scores, _params(**dict(kw, softmax_reg=reg)), neigh, pv)
+        assert code[FLAGS[out.flag]] == int(gold["flag"][trial]), (trial, FLAGS[out.flag], int(gold["flag"][trial]))
+        assert out.scale_ind == int(gold["scale_ind"][trial]), (trial, out.scale_ind, int(gold["scale_ind"][trial]))
+        cell = (out.r2, out.c2) if out.use_second else (out.r1, out.c1)
+        mine = (torch.Tensor(cell) - 9) * (img_support_sz / out_sz) * sample_scales[out.scale_ind]
+        assert torch.equal(mine, torch.from_numpy(gold["translation"][trial])), (trial, mine, gold["translation"][trial])

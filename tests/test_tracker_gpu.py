@@ -133,6 +133,26 @@ def test_localize_kernel_matches_reference_code_on_random_maps():
     assert {("normal", 0), ("hard_negative", 0), ("hard_negative", 1), ("uncertain", 0), ("not_found", 0), (None, 0)} <= seen, seen
 
 
+def test_localize_kernel_matches_reference_code_on_nan_maps():
+    """NaN in the score maps (tests/tracker_cases.py:nan_localize_cases, no pre-processing, 'exp' and 'softmax') against the reference's
+    `localize_target` on the same problems (tests/golden/dimp_localize_nan.npz): flag, scale index and translation exactly."""
+    from tracker_cases import nan_localize_cases
+    from pytracking_b200.tracker import FLAGS
+    gold = np.load(os.path.join(GOLDEN, "dimp_localize_nan.npz"))
+    code = {None: 0, "normal": 1, "hard_negative": 2, "uncertain": 3, "not_found": 4}
+    img_support_sz, out_sz = torch.Tensor([288, 288]), torch.Tensor([18, 18])
+    for trial, kw, reg, scores, target_sz, sample_scales, sample_pos, pos in nan_localize_cases():
+        S = scores.shape[0]
+        neigh = [(2.2 * (target_sz / sample_scales[s]) * (out_sz / img_support_sz)).numpy() for s in range(S)]
+        pv = [((pos - sample_pos[s]) / ((img_support_sz / out_sz) * sample_scales[s])).numpy() for s in range(S)]
+        out = _run_localize(scores, _params(**dict(kw, softmax_reg=reg)), neigh, pv)
+        assert code[FLAGS[out.flag]] == int(gold["flag"][trial]), (trial, FLAGS[out.flag], int(gold["flag"][trial]))
+        assert out.scale_ind == int(gold["scale_ind"][trial]), (trial, out.scale_ind, int(gold["scale_ind"][trial]))
+        cell = (out.r2, out.c2) if out.use_second else (out.r1, out.c1)
+        mine = (torch.Tensor(cell) - 9) * (img_support_sz / out_sz) * sample_scales[out.scale_ind]
+        assert torch.equal(mine, torch.from_numpy(gold["translation"][trial])), (trial, mine, gold["translation"][trial])
+
+
 # ---------------------------------------------------------------------------------------------------------------------------
 def test_native_tracker_reproduces_recorded_reference_run():
     """Native initialisation + 40 closed-loop frames from uint8 frames: boxes bit-identical to the reference tracker's (CPU,

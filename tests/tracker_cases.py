@@ -43,6 +43,52 @@ def random_localize_cases(n=400):
         yield trial, kw, scores, target_sz, sample_scales, sample_pos, pos
 
 
+def nan_localize_cases():
+    """Seeded localisation problems with NaN in the score maps: yields (trial, params overrides, softmax_reg, scores [S,19,19], target_sz,
+    sample_scales, sample_pos, pos).  One NaN cell inside and outside the target neighbourhood, a NaN column, a NaN scale among finite
+    ones, an all-NaN map, with and without advanced localisation and through the 'exp' and 'softmax' pre-processing.  The reference's
+    answers are tests/golden/dimp_localize_nan.npz (oracle/gen_host_logic_golden.py localize_nan)."""
+    import torch
+    g = torch.Generator().manual_seed(3)
+    nan = float("nan")
+    kinds = ("inside", "outside", "column", "scale", "all", "two")
+    pres = ((None, "none"), (None, "exp"), (None, "softmax"), (1.5, "softmax"))
+    trial = 0
+    for kind in kinds:
+        for j in range(4):
+            S = 1 + (trial % 3) if kind != "scale" else 2 + j % 2
+            reg, pre = pres[j] if kind in ("inside", "all", "column") else pres[j % 2]
+            kw = dict(advanced_localization=j != 3 or kind == "scale", target_not_found_threshold=0.2 if pre == "none" else 0.01,
+                      uncertain_threshold=-float("inf"), hard_sample_threshold=-float("inf"), distractor_threshold=0.8,
+                      hard_negative_threshold=0.5, dispalcement_scale=0.3 + 0.5 * (trial % 2), score_preprocess=pre)
+            scores = 0.1 * torch.rand(S, 19, 19, generator=g)
+            peaks = []
+            for s in range(S):
+                r, c = [int(v) for v in torch.randint(2, 17, (2,), generator=g)]
+                scores[s, r, c] = 0.3 + 0.5 * float(torch.rand(1, generator=g))
+                peaks.append((r, c))
+            s0 = int(torch.randint(0, S, (1,), generator=g))
+            r, c = peaks[s0]
+            if kind == "inside":
+                scores[s0, r + 1, c - 1] = nan
+            elif kind == "outside":
+                scores[s0, (r + 9) % 19, (c + 9) % 19] = nan
+            elif kind == "column":
+                scores[s0, :, (c + 7) % 19] = nan
+            elif kind == "scale":
+                scores[S - 1, 4 + j, 3] = nan
+            elif kind == "all":
+                scores[s0] = nan
+            else:
+                scores[s0, 2, 5] = scores[s0, 14, 5] = scores[s0, 9, 12] = nan
+            target_sz = torch.Tensor([60, 80]) * (0.5 + float(torch.rand(1, generator=g)))
+            sample_scales = 1.0 + 0.5 * torch.rand(S, generator=g)
+            sample_pos = torch.Tensor([[240, 320]]).repeat(S, 1) + torch.rand(S, 2, generator=g)
+            pos = sample_pos[0] + 40 * (torch.rand(2, generator=g) - 0.5)
+            yield trial, kw, reg, scores, target_sz, sample_scales, sample_pos, pos
+            trial += 1
+
+
 def _loc(d, t):
     loc = _lib.LocResult()
     loc.flag, loc.scale_ind = int(d["flag"][t]), 0
