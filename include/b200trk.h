@@ -247,7 +247,11 @@ typedef struct {
  *   omitted altogether (backbone descriptors only, e.g. ATOM's ATOMResNet18 features): dims[6..8] are then 0 and `clf` must be NULL.
  *   norm_scale: InstanceL2Norm scale (sqrt(1/(out_dim*filter_size^2)), ltr/models/tracking/dimpnet.py:159).
  *   max_batch: largest S the handle will be run with (13 at DiMP.initialize, 1 per frame).
- *   precision: 0 = fp32-faithful (error-compensated 3xTF32 tensor-core MMA + fp32 CUDA-core stem), 1 = fp32 CUDA cores only. */
+ *   precision: 0 = fp32-faithful (error-compensated 3xTF32 tensor-core MMA + fp32 CUDA-core stem), 1 = fp32 CUDA cores only,
+ *   2 = single-pass TF32 on the tensor cores (both operands rounded once to TF32 with cvt.rna, one MMA per K step, fp32 accumulation;
+ *   the stem, max-pool, InstanceL2Norm and every convolution the tensor-core kernel does not take run as at 0). Any other value is
+ *   refused before anything is allocated. The IoU branch, filter_conv and conv3_1r / conv4_1r attached later follow the handle's
+ *   precision; b200trk_net_op_weights returns the raw fp32 weights at every precision. */
 int b200trk_net_create(b200trk_net_t** out, int arch, const b200trk_conv_desc_t* convs, int n_convs,
                        float norm_scale, int max_batch, int crop_h, int crop_w, int precision);
 int b200trk_net_destroy(b200trk_net_t* net);
@@ -378,7 +382,9 @@ int b200trk_tomp_tokens(const float* train_feat, const float* test_feat, const f
 
 /* ToMP bounding-box regression tower -- DenseBoxRegressor.forward after the filter projection (ltr/models/transformer/heads.py:118-141):
  * feats_att = attention * feat; n_convs - 1 times [conv3x3 + GroupNorm(1, C) + ReLU] (heads.py:8-15); conv3x3 -> 4; exp.
- * convs: HOST descriptors (3x3, stride 1, pad 1, bias, no BN) in execution order; gn_gamma / gn_beta: n_convs - 1 HOST [C] vectors. */
+ * convs: HOST descriptors (3x3, stride 1, pad 1, bias, no BN) in execution order; gn_gamma / gn_beta: n_convs - 1 HOST [C] vectors.
+ * precision: as b200trk_net_create (0 = 3xTF32, 1 = fp32 CUDA cores, 2 = single-pass TF32 on the tensor cores); any other value is
+ * refused before anything is allocated. */
 typedef struct b200trk_tower b200trk_tower_t;
 int b200trk_tower_create(b200trk_tower_t** out, const b200trk_conv_desc_t* convs, int n_convs, const float* const* gn_gamma,
                          const float* const* gn_beta, int C, int H, int W, int max_batch, int precision);

@@ -27,6 +27,12 @@
 // reduces its share of the tile through distributed shared memory in split order (fixed order => bitwise deterministic); with more
 // than 8 splits, when the device cannot hold all of the grid's clusters at once, or with B200TRK_TC_CLUSTER=0, the partial tiles go
 // to an L2-resident workspace and a per-tile arrival counter releases the split CTAs.
+//
+// Single-pass TF32 (plan precision 2, conv_tc_kernel<BN + TC_SINGLE>): every operand is rounded once to TF32 (cvt.rna, the hi half
+// of the split) and each K step is one MMA into one accumulator set. The weights are rounded once when the plan is built into a [Cout][K] copy
+// (B = one box {32, BN, 1}); A is rounded in registers as its fragments are loaded. With 64 accumulators instead of 128, BN = 128
+// takes A from registers like BN = 64, so no thread writes the stages at either width: stage = A (raw) | B, 24 KB (BN 64, 8
+// stages) or 32 KB (BN 128, 6 stages). Tiling, split-K, the epilogue, PDL and the debug stamps are those of the 3xTF32 kernel.
 #include "net.cuh"
 #include "tc_ptx.cuh"
 #include <cuda.h>
@@ -40,10 +46,11 @@ constexpr int TC_KB = 32;                   // fp32 elements per 128-byte K bloc
 constexpr int TC_CT = 256;                  // consumer threads (warps 0-7)
 constexpr int TC_THREADS = TC_CT + 32;      // + the TMA producer warp
 constexpr int TC_MAX_STAGES = 6;
+constexpr int TC1_MAX_STAGES = 8;           // single-pass TF32: 8 x 24 KB stages at BN = 64
 constexpr int TC_SMEM_MAX = 220 * 1024;
 
 struct TcParams {
-    CUtensorMap a_map, b_map;       // raw fp32 activations (4-D) and TF32-split weights (3-D: K, Cout, hi | lo)
+    CUtensorMap a_map, b_map;       // raw fp32 activations (4-D) and TF32 weights (3-D: K, Cout, hi | lo or the one rounded copy)
     float* out_raw;
     const float* bias; const float* residual;
     float* ws; unsigned* counters;
@@ -57,12 +64,14 @@ struct TcParams {
     int cluster_red; // 1: the split-K CTAs of a tile form a thread-block cluster (1,1,splits) and reduce their partial tiles through
                      //    distributed shared memory instead of an L2 workspace + arrival counter
     uint32_t stage_bytes;
-    uint32_t a_bytes, b_bytes;      // bytes one k-block's TMA lands: the A box | the B_hi and B_lo tiles
+    uint32_t a_bytes, b_bytes;      // bytes one k-block's TMA lands: the A box | the B_hi and B_lo tiles (single pass: the B tile)
 };
 
 struct TcConv {
     TcParams P;
-    float* w_split = nullptr;       // [2][Cout][K]: TF32 hi | lo of the weights, the B operand (owned by the plan)
+    float* w_split = nullptr;       // the B operand (owned by the plan): [2][Cout][K] TF32 hi | lo of the weights, or, single pass,
+                                    // [Cout][K] the weights rounded to TF32
+    int single = 0;                 // 1: single-pass TF32 (plan precision 2, conv_tc_kernel<BN + TC_SINGLE>)
     int S_built = 0;
 };
 
@@ -104,19 +113,30 @@ __global__ void tc_split_weights_kernel(const float* __restrict__ w, float* __re
     }
 }
 
-template <int BN>
+// single-pass TF32: the weights rounded once per plan, w1[i] = the hi half of w[i]'s split
+__global__ void tc_round_weights_kernel(const float* __restrict__ w, float* __restrict__ w1, size_t n) {
+    for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x) w1[i] = tf32_rna(w[i]);
+}
+
+// One template for both products. The argument V is the tile width BN for 3xTF32, or BN + TC_SINGLE for single-pass TF32, so that the
+// 3xTF32 instances keep the symbols (and the code) they had before the single-pass variant existed.
+constexpr int TC_SINGLE = 1;
+template <int V>
 __global__ void __launch_bounds__(TC_THREADS, 1) conv_tc_kernel(const __grid_constant__ TcParams P) {
+    constexpr int BN = V & ~TC_SINGLE;
+    constexpr bool SINGLE = (V & TC_SINGLE) != 0;
     constexpr int NACC = BN / 2;                 // accumulator registers per thread and product group
     constexpr uint32_t a_tile = (uint32_t)TC_BM * 128u;   // 16 KB slot regardless of the box size
     constexpr uint32_t b_tile = (uint32_t)BN * 128u;
     // BN = 64: A from registers, stage = A (raw) | B_hi | B_lo. BN = 128: A from shared memory, split in place by the warpgroup that
-    // reads it, stage = A_hi | A_lo | B_hi | B_lo (see the header)
-    constexpr bool a_smem = BN == 128;
+    // reads it, stage = A_hi | A_lo | B_hi | B_lo (see the header). Single pass: A from registers at both widths, stage = A (raw) | B
+    constexpr bool a_smem = BN == 128 && !SINGLE;
     constexpr uint32_t b_off = (a_smem ? 2u : 1u) * a_tile;
     constexpr int RP = BN + 4;                   // floats per staged accumulator row (conflict-free 128-bit accesses)
+    constexpr int MAX_STAGES = SINGLE ? TC1_MAX_STAGES : TC_MAX_STAGES;
     extern __shared__ uint8_t tc_smem_raw[];
-    __shared__ __align__(8) uint64_t s_full[TC_MAX_STAGES];
-    __shared__ __align__(8) uint64_t s_empty[TC_MAX_STAGES];
+    __shared__ __align__(8) uint64_t s_full[MAX_STAGES];
+    __shared__ __align__(8) uint64_t s_empty[MAX_STAGES];
 
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     uint8_t* sbase = tc_smem_raw + ((1024u - (smem_u32(tc_smem_raw) & 1023u)) & 1023u);
@@ -192,7 +212,37 @@ __global__ void __launch_bounds__(TC_THREADS, 1) conv_tc_kernel(const __grid_con
         float acc[NACC], acc2[NACC];                  // A_hi*B_hi | A_lo*B_hi + A_hi*B_lo
 #pragma unroll
         for (int i = 0; i < NACC; ++i) { acc[i] = 0.f; acc2[i] = 0.f; }
-        if constexpr (!a_smem) {
+        if constexpr (SINGLE) {
+            // one set of rounded A fragments per k-block, two sets alternating as in the 3xTF32 BN = 64 loop; 4 MMAs per k-block
+            uint32_t a0[4][4], a1[4][4];
+            int st = 0, prev = 0;
+            uint32_t ph = 0;
+            auto step = [&](int it, const uint32_t (&a)[4][4], uint32_t (&na)[4][4]) {
+                const uint32_t sb = smem_base + (uint32_t)st * stage_bytes + b_off;
+                wgmma_fence();
+#pragma unroll
+                for (int k = 0; k < TC_KB / 8; ++k) {
+                    if constexpr (BN == 64) wgmma_rs_n64(acc, a[k], wg_desc(sb + (uint32_t)k * 32u));
+                    else wgmma_rs_n128(acc, a[k], wg_desc(sb + (uint32_t)k * 32u));
+                }
+                wgmma_commit();
+                wgmma_wait<1>();
+                if (it > 0 && lane == 0) mbar_arrive(smem_u32(&s_empty[prev]));
+                prev = st;
+                if (++st == P.stages) { st = 0; ph ^= 1u; }
+                if (it + 1 < nkb) {
+                    mbar_wait(smem_u32(&s_full[st]), ph);
+                    load_frags_tf32(sbase + (size_t)st * stage_bytes, r0, kq, na);
+                }
+            };
+            mbar_wait(smem_u32(&s_full[0]), 0);
+            if (dbg && ct == 0) dbg[3] = gtimer();                            // first operands landed
+            load_frags_tf32(sbase, r0, kq, a0);
+            for (int it = 0; it < nkb; it += 2) {
+                step(it, a0, a1);
+                if (it + 1 < nkb) step(it + 1, a1, a0);
+            }
+        } else if constexpr (!a_smem) {
             uint32_t ah0[4][4], al0[4][4], ah1[4][4], al1[4][4];    // two sets of A fragments (4 K steps), alternating by k-block
             int st = 0, prev = 0;
             uint32_t ph = 0;
@@ -266,7 +316,8 @@ __global__ void __launch_bounds__(TC_THREADS, 1) conv_tc_kernel(const __grid_con
             }
         }
         wgmma_wait<0>();
-        wg_reg_fence(acc); wg_reg_fence(acc2);
+        wg_reg_fence(acc);
+        if constexpr (!SINGLE) wg_reg_fence(acc2);
         if (dbg && ct == 0) dbg[4] = gtimer();                            // accumulator complete
         asm volatile("bar.sync 1, %0;" ::"n"(TC_CT) : "memory");              // every wgmma of both warpgroups has read its operands
         {
@@ -274,9 +325,13 @@ __global__ void __launch_bounds__(TC_THREADS, 1) conv_tc_kernel(const __grid_con
 #pragma unroll
             for (int j = 0; j < BN / 8; ++j)
 #pragma unroll
-                for (int h = 0; h < 2; ++h)
-                    *reinterpret_cast<float2*>(red + (r0 + 8 * h) * RP + 8 * j + c0) =
-                        make_float2(acc[4 * j + 2 * h] + acc2[4 * j + 2 * h], acc[4 * j + 2 * h + 1] + acc2[4 * j + 2 * h + 1]);
+                for (int h = 0; h < 2; ++h) {
+                    if constexpr (SINGLE)
+                        *reinterpret_cast<float2*>(red + (r0 + 8 * h) * RP + 8 * j + c0) = make_float2(acc[4 * j + 2 * h], acc[4 * j + 2 * h + 1]);
+                    else
+                        *reinterpret_cast<float2*>(red + (r0 + 8 * h) * RP + 8 * j + c0) =
+                            make_float2(acc[4 * j + 2 * h] + acc2[4 * j + 2 * h], acc[4 * j + 2 * h + 1] + acc2[4 * j + 2 * h + 1]);
+                }
         }
     }
     __syncthreads();                              // the staged tile is complete
@@ -382,6 +437,12 @@ __global__ void __launch_bounds__(TC_THREADS, 1) conv_tc_kernel(const __grid_con
     if (dbg && threadIdx.x == 0) dbg[6] = gtimer();                       // epilogue done
 }
 
+typedef void (*TcKernel)(TcParams);
+static TcKernel tc_kernel(int BN, int single) {
+    if (single) return BN == 64 ? conv_tc_kernel<64 + TC_SINGLE> : conv_tc_kernel<128 + TC_SINGLE>;
+    return BN == 64 ? conv_tc_kernel<64> : conv_tc_kernel<128>;
+}
+
 // ------------------------------------------------------------------------------------------------------------
 // host side
 // ------------------------------------------------------------------------------------------------------------
@@ -481,15 +542,17 @@ int tc_conv_prepare(b200trk_net* net, Op& op, const std::vector<float>& w_khwc) 
     B200_CHECK_CUDA(cudaMemset(cnt, 0, 1024 * sizeof(unsigned)));
     net->owned.push_back(cnt);
     P.counters = (unsigned*)cnt;
-    // The B operand: the weights split into TF32 hi | lo once, here, instead of in every CTA that loads them. op.w stays the raw
-    // fp32 weights (the plan's weight read-back and the exact-fp32 path use them).
+    // The B operand: the weights split into TF32 hi | lo (precision 2: rounded to TF32) once, here, instead of in every CTA that
+    // loads them. op.w stays the raw fp32 weights (the plan's weight read-back and the exact-fp32 path use them).
+    tc->single = net->precision == 2;
     const size_t nw = (size_t)op.Cout * op.k * op.k * op.Cin;
     void* hl = nullptr;
-    B200_CHECK_CUDA(cudaMalloc(&hl, 2 * nw * sizeof(float)));
+    B200_CHECK_CUDA(cudaMalloc(&hl, (tc->single ? 1 : 2) * nw * sizeof(float)));
     net->owned.push_back(hl);
     tc->w_split = (float*)hl;
     const size_t blocks = (nw + 255) / 256;
-    tc_split_weights_kernel<<<(unsigned)(blocks < 4096 ? blocks : 4096), 256>>>(op.w, tc->w_split, nw);
+    if (tc->single) tc_round_weights_kernel<<<(unsigned)(blocks < 4096 ? blocks : 4096), 256>>>(op.w, tc->w_split, nw);
+    else tc_split_weights_kernel<<<(unsigned)(blocks < 4096 ? blocks : 4096), 256>>>(op.w, tc->w_split, nw);
     B200_CHECK_CUDA(cudaGetLastError());
     B200_CHECK_CUDA(cudaStreamSynchronize(0));
     tc->S_built = -1;
@@ -501,6 +564,8 @@ static int tc_set_kernel_attrs() {
     if (!attr) {
         B200_CHECK_CUDA(cudaFuncSetAttribute(conv_tc_kernel<64>, cudaFuncAttributeMaxDynamicSharedMemorySize, TC_SMEM_MAX));
         B200_CHECK_CUDA(cudaFuncSetAttribute(conv_tc_kernel<128>, cudaFuncAttributeMaxDynamicSharedMemorySize, TC_SMEM_MAX));
+        B200_CHECK_CUDA(cudaFuncSetAttribute(conv_tc_kernel<64 + TC_SINGLE>, cudaFuncAttributeMaxDynamicSharedMemorySize, TC_SMEM_MAX));
+        B200_CHECK_CUDA(cudaFuncSetAttribute(conv_tc_kernel<128 + TC_SINGLE>, cudaFuncAttributeMaxDynamicSharedMemorySize, TC_SMEM_MAX));
         attr = true;
     }
     return 0;
@@ -515,7 +580,7 @@ static size_t tc_smem_bytes(const TcParams& P) {
 // How many (1, 1, splits) clusters of this configuration the device can hold at once. A cluster's CTAs must share a GPC, so
 // sizes that do not divide a GPC's SM count leave SMs idle: on a 132-SM H100, 44 clusters of 3 or 24 of 5 do not all fit, and
 // the last clusters run as a second wave that costs a whole CTA lifetime.
-static int tc_max_active_clusters(const TcParams& P, int ctas, int* n) {
+static int tc_max_active_clusters(const TcParams& P, int single, int ctas, int* n) {
     if (int e = tc_set_kernel_attrs()) return e;
     cudaLaunchConfig_t cfg;
     memset(&cfg, 0, sizeof(cfg));
@@ -524,8 +589,7 @@ static int tc_max_active_clusters(const TcParams& P, int ctas, int* n) {
     at.id = cudaLaunchAttributeClusterDimension;
     at.val.clusterDim.x = 1; at.val.clusterDim.y = 1; at.val.clusterDim.z = (unsigned)P.splits;
     cfg.attrs = &at; cfg.numAttrs = 1;
-    if (P.BN == 64) B200_CHECK_CUDA(cudaOccupancyMaxActiveClusters(n, conv_tc_kernel<64>, &cfg));
-    else B200_CHECK_CUDA(cudaOccupancyMaxActiveClusters(n, conv_tc_kernel<128>, &cfg));
+    B200_CHECK_CUDA(cudaOccupancyMaxActiveClusters(n, tc_kernel(P.BN, single), &cfg));
     return 0;
 }
 
@@ -550,12 +614,15 @@ static int tc_configure(b200trk_net* net, const Op& op, TcConv* tc, int S) {
     }
     if (op.Cout % BN != 0 || (BN != 64 && BN != 128)) BN = 64;
     P.BN = BN;
-    P.b_bytes = 2u * (uint32_t)BN * 128u;                           // B_hi | B_lo
-    // BN 64: A | B_hi | B_lo, 32 KB (6 stages); BN 128: A_hi | A_lo | B_hi | B_lo, 64 KB (3 stages)
-    const uint32_t stage_bytes = (BN == 128 ? 2u : 1u) * TC_BM * 128u + P.b_bytes;
+    const uint32_t nb = tc->single ? 1u : 2u;
+    P.b_bytes = nb * (uint32_t)BN * 128u;                           // B_hi | B_lo, or the rounded B
+    // BN 64: A | B_hi | B_lo, 32 KB (6 stages); BN 128: A_hi | A_lo | B_hi | B_lo, 64 KB (3 stages).
+    // Single pass: A | B, 24 KB (BN 64, 8 stages) or 32 KB (BN 128, 6 stages).
+    const uint32_t stage_bytes = (BN == 128 && !tc->single ? 2u : 1u) * TC_BM * 128u + P.b_bytes;
     P.stage_bytes = stage_bytes;
+    const int max_stages = tc->single ? TC1_MAX_STAGES : TC_MAX_STAGES;
     int stages = (int)((TC_SMEM_MAX - 1024u) / stage_bytes);
-    if (stages > TC_MAX_STAGES) stages = TC_MAX_STAGES;
+    if (stages > max_stages) stages = max_stages;
     if (stages > P.total_kb) stages = P.total_kb;
     if (stages < 2) stages = 2;
     P.stages = stages;
@@ -581,14 +648,14 @@ static int tc_configure(b200trk_net* net, const Op& op, TcConv* tc, int S) {
         // reductions add the same staged partial tiles in split order from 0.f, padded with zeros to 8 terms, so the output is
         // bitwise the same.
         int fit = 0;
-        if (int e = tc_max_active_clusters(P, ctas, &fit)) return e;
+        if (int e = tc_max_active_clusters(P, tc->single, ctas, &fit)) return e;
         if (fit < ctas) P.cluster_red = 0;
     }
-    // {K, Cout, hi | lo}: one box {32, BN, 2} lands B_hi and, BN * 128 bytes behind it, B_lo
+    // {K, Cout, hi | lo}: one box {32, BN, 2} lands B_hi and, BN * 128 bytes behind it, B_lo (single pass: {K, Cout, 1}, box {32, BN, 1})
     const uint64_t Kt = (uint64_t)op.k * op.k * op.Cin;
-    const uint64_t bdims[3] = {Kt, (uint64_t)op.Cout, 2};
+    const uint64_t bdims[3] = {Kt, (uint64_t)op.Cout, nb};
     const uint64_t bstrides[2] = {Kt * sizeof(float), Kt * op.Cout * sizeof(float)};
-    const uint32_t bbox[3] = {TC_KB, (uint32_t)BN, 2};
+    const uint32_t bbox[3] = {TC_KB, (uint32_t)BN, nb};
     if (int e = tc_make_map(&P.b_map, tc->w_split, 3, bdims, bstrides, bbox, 1)) return e;
     tc->S_built = S;
     return 0;
@@ -615,8 +682,7 @@ int tc_conv_launch(b200trk_net* net, const Op& op, int S, cudaStream_t st) {
         ++nat;
     }
     cfg.attrs = at; cfg.numAttrs = nat;
-    if (P.BN == 64) B200_CHECK_CUDA(cudaLaunchKernelEx(&cfg, conv_tc_kernel<64>, P));
-    else B200_CHECK_CUDA(cudaLaunchKernelEx(&cfg, conv_tc_kernel<128>, P));
+    B200_CHECK_CUDA(cudaLaunchKernelEx(&cfg, tc_kernel(P.BN, tc->single), P));
     B200_LAUNCH_CHECK();
     return 0;
 }

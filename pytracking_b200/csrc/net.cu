@@ -77,7 +77,7 @@ struct Builder {
             B200_CHECK_CUDA(cudaMemcpy(op.bias, b.data(), b.size() * sizeof(float), cudaMemcpyHostToDevice));
         }
         if (int e = new_buf(net, (size_t)op.Hout * op.Wout * cout, &op.out)) return e;
-        if (net->precision == 0 && tc_conv_supported(op)) {
+        if (net->precision != 1 && tc_conv_supported(op)) {
             if (int e = tc_conv_prepare(net, op, w)) return e;
         }
         net->flops += 2.0 * (double)op.Hout * op.Wout * cout * (double)k * k * cin;
@@ -196,7 +196,8 @@ extern "C" int b200trk_net_create(b200trk_net_t** out, int arch, const b200trk_c
     B200_REQUIRE(max_batch >= 1 && max_batch <= 64, "net_create: max_batch=%d out of range", max_batch);
     B200_REQUIRE(crop_h >= 32 && crop_w >= 32 && crop_h % 16 == 0 && crop_w % 16 == 0,
                  "net_create: crop %dx%d must be a multiple of 16", crop_h, crop_w);
-    B200_REQUIRE(precision == 0 || precision == 1, "net_create: precision must be 0 (3xTF32 tensor cores) or 1 (fp32 CUDA cores)");
+    B200_REQUIRE(precision >= 0 && precision <= 2,
+                 "net_create: precision %d must be 0 (3xTF32 tensor cores), 1 (fp32 CUDA cores) or 2 (TF32 tensor cores)", precision);
     b200trk_net* net = new b200trk_net();
     net->arch = arch; net->crop_h = crop_h; net->crop_w = crop_w; net->max_batch = max_batch; net->precision = precision;
     net->norm_scale = norm_scale;

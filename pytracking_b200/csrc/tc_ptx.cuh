@@ -1,6 +1,6 @@
 // PTX wrappers shared by the Hopper tensor-core kernels (conv_tc.cu, sd_tc.cu): mbarrier, TMA tensor loads, warpgroup MMAs
 // (wgmma.mma_async, TF32 in / FP32 accumulate in registers), the K-major SWIZZLE_128B shared-memory descriptor, the split used
-// for 3xTF32 and the register-A fragment load that applies it.
+// for 3xTF32 and the register-A fragment loads that apply it (or, single-pass TF32, only its rounding).
 #pragma once
 #include "common.cuh"
 #include <cuda.h>
@@ -111,6 +111,13 @@ __device__ __forceinline__ void wgmma_ss_n128(float (&d)[64], uint64_t adesc, ui
                  : "l"(adesc), "l"(bdesc) : "memory");
 }
 
+__device__ __forceinline__ void wgmma_rs_n128(float (&d)[64], const uint32_t (&a)[4], uint64_t bdesc) {
+    asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, 1, 0;\n\twgmma.mma_async.sync.aligned.m64n128k8.f32.tf32.tf32 "
+                 "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, {%64, %65, %66, %67}, %68, p, 1, 1;\n\t}"
+                 : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+                 : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(bdesc) : "memory");
+}
+
 __device__ __forceinline__ void wgmma_rs_n16(float (&d)[8], const uint32_t (&a)[4], uint64_t bdesc) {
     asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, 1, 0;\n\twgmma.mma_async.sync.aligned.m64n16k8.f32.tf32.tf32 "
                  "{%0, %1, %2, %3, %4, %5, %6, %7}, {%8, %9, %10, %11}, %12, p, 1, 1;\n\t}"
@@ -146,6 +153,20 @@ __device__ __forceinline__ void load_frags_split(const uint8_t* sb, int r0, int 
             split_tf32(x[ks][r], h, l);
             ah[ks][r] = __float_as_uint(h); al[ks][r] = __float_as_uint(l);
         }
+}
+// The same fragments of a K-major swizzled tile, each rounded once to TF32 (cvt.rna, the hi half of the split): single-pass TF32.
+template <int NKS>
+__device__ __forceinline__ void load_frags_tf32(const uint8_t* sb, int r0, int kq, uint32_t (&a)[NKS][4]) {
+    float x[NKS][4];
+#pragma unroll
+    for (int ks = 0; ks < NKS; ++ks)
+#pragma unroll
+        for (int r = 0; r < 4; ++r)
+            x[ks][r] = *reinterpret_cast<const float*>(sb + sw128(r0 + 8 * (r & 1), 8 * ks + kq + 4 * (r >> 1)));
+#pragma unroll
+    for (int ks = 0; ks < NKS; ++ks)
+#pragma unroll
+        for (int r = 0; r < 4; ++r) a[ks][r] = __float_as_uint(tf32_rna(x[ks][r]));
 }
 
 // Host: fp32 tensor map (element strides 1, zero OOB fill) of rank 2..4, SWIZZLE_128B (box[0] = 32) or no swizzle; `strides_bytes`

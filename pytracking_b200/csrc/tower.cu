@@ -42,6 +42,8 @@ extern "C" int b200trk_tower_create(b200trk_tower_t** out, const b200trk_conv_de
                                     const float* const* gn_beta, int C, int H, int W, int max_batch, int precision) {
     B200_REQUIRE(out && convs && gn_gamma && gn_beta, "tower_create: null pointer");
     B200_REQUIRE(n_convs >= 2 && n_convs <= 9 && C % 32 == 0 && H > 0 && W > 0 && max_batch >= 1 && max_batch <= 16, "tower_create: bad shape");
+    B200_REQUIRE(precision >= 0 && precision <= 2,
+                 "tower_create: precision %d must be 0 (3xTF32 tensor cores), 1 (fp32 CUDA cores) or 2 (TF32 tensor cores)", precision);
     b200trk_tower* t = new b200trk_tower();
     b200trk_net* net = &t->net;
     net->max_batch = max_batch; net->precision = precision; net->crop_h = H; net->crop_w = W; net->sms = device_sm_count();
@@ -73,7 +75,7 @@ extern "C" int b200trk_tower_create(b200trk_tower_t** out, const b200trk_conv_de
         float* ob = nullptr;
         if (!e) e = tower_alloc(net, &ob, (size_t)max_batch * H * W * d.cout);
         if (!e) { net->bufs.push_back(ob); net->buf_floats.push_back((size_t)H * W * d.cout); op.out = (int)net->bufs.size() - 1; }
-        if (!e && precision == 0 && tc_conv_supported(op)) e = tc_conv_prepare(net, op, w);
+        if (!e && precision != 1 && tc_conv_supported(op)) e = tc_conv_prepare(net, op, w);
         if (!e) {
             net->flops += 2.0 * H * W * (double)d.cout * 9.0 * d.cin;
             net->ops.push_back(op);

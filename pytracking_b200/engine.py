@@ -68,7 +68,10 @@ def conv_descs_from_state_dict(sd, arch, backbone_prefix="feature_extractor.", h
 
 
 class BackboneEngine:
-    """Owns a `b200trk_net_t`. forward(im) mirrors NetWithBackbone.extract_backbone + extract_classification_feat."""
+    """Owns a `b200trk_net_t`. forward(im) mirrors NetWithBackbone.extract_backbone + extract_classification_feat.
+    `precision`: 0 = 3xTF32 on the tensor cores (fp32-faithful), 1 = exact fp32 on the CUDA cores, 2 = single-pass TF32 on the tensor
+    cores (each operand rounded once to TF32, fp32 accumulation: the numerics cuDNN gives a PyTorch convolution with TF32 allowed).
+    The precision covers every convolution of the plan, the heads attached later included."""
 
     def __init__(self, state_dict, arch="resnet50", filter_size=4, max_batch=1, crop_size=288, precision=0, device=None, head=True,
                  head_prefix="classifier.feature_extractor.", norm_scale=None):

@@ -969,7 +969,9 @@ def install(max_batch=16, precision=0, skip=()):
     """`skip`: attribute names (e.g. "predict_iou" or "AtomIoUNet.predict_iou") to leave on the reference implementation.
     Rebind the seams inside an importable pytracking / ltr checkout (no reference file is edited); `uninstall()` restores them.
     Calls the CUDA path does not claim (CPU tensors, autograd, training mode, shapes the library rejects) fall through to the
-    reference implementation. Returns the list of rebound attributes."""
+    reference implementation. Returns the list of rebound attributes.
+    `precision` (0, 1 or 2, see `engine.BackboneEngine`) applies to the convolution plans: the backbones, their heads and the ToMP
+    box tower. precision=2 leaves the ToMP transformer, the filter optimisers and the correlation kernels as they are at 0."""
     global _state
     if not _installed:
         _state = _State(max_batch, precision)

@@ -1,4 +1,4 @@
-"""Per-layer phase timing of the tensor-core plan from in-kernel globaltimer stamps (warm, back-to-back launches).
+"""python tools/tc_phases.py [S] [precision]: per-layer phase timing of the tensor-core plan from in-kernel globaltimer stamps (warm, back-to-back launches).
 
 Stamps per CTA: 0 start, 1 prologue done, 2 previous grid complete, 3 first operands landed, 4 accumulator complete,
 5 all splits staged / arrived, 6 epilogue done.
@@ -13,10 +13,11 @@ from pytracking_b200 import synth, _lib
 from pytracking_b200.engine import BackboneEngine
 
 S = int(sys.argv[1]) if len(sys.argv) > 1 else 1
+PRECISION = int(sys.argv[2]) if len(sys.argv) > 2 else 0       # 0: 3xTF32, 2: single-pass TF32
 sd = synth.make_dimp_state_dict("resnet50", seed=0, lut_seed=3)
 im = synth.make_crop(41, S, 288).cuda()
 L = _lib.lib()
-eng = BackboneEngine(sd, arch="resnet50", max_batch=S, crop_size=288, precision=0)
+eng = BackboneEngine(sd, arch="resnet50", max_batch=S, crop_size=288, precision=PRECISION)
 for _ in range(3):
     eng.forward(im, want=("classification",))
 n = L.b200trk_net_num_ops(eng.handle)
