@@ -62,6 +62,47 @@ int device_sm_count() {
     return g_sm_count[dev];
 }
 
+Owner::~Owner() {
+    for (void* p : dev_) cudaFree(p);
+    for (void* p : host_) cudaFreeHost(p);
+    for (cudaEvent_t ev : events_) cudaEventDestroy(ev);
+}
+
+int Owner::alloc(void** p, size_t bytes, bool zero) {
+    B200_CHECK_CUDA(cudaMalloc(p, bytes));
+    dev_.push_back(*p);
+    if (zero) B200_CHECK_CUDA(cudaMemset(*p, 0, bytes));
+    return 0;
+}
+
+int Owner::upload(void** p, const void* host, size_t bytes) {
+    if (int e = alloc(p, bytes, false)) return e;
+    B200_CHECK_CUDA(cudaMemcpy(*p, host, bytes, cudaMemcpyHostToDevice));
+    return 0;
+}
+
+int Owner::pinned(void** p, size_t bytes) {
+    B200_CHECK_CUDA(cudaMallocHost(p, bytes));
+    host_.push_back(*p);
+    return 0;
+}
+
+int Owner::event(cudaEvent_t* ev, unsigned flags) {
+    B200_CHECK_CUDA(cudaEventCreateWithFlags(ev, flags));
+    events_.push_back(*ev);
+    return 0;
+}
+
+int Owner::release(void* p) {
+    for (size_t i = 0; i < dev_.size(); ++i)
+        if (dev_[i] == p) {
+            dev_.erase(dev_.begin() + i);
+            B200_CHECK_CUDA(cudaFree(p));
+            return 0;
+        }
+    return 0;
+}
+
 }  // namespace b200trk
 
 // debug: copy the SD optimiser phase trace (128 x u64) to the host

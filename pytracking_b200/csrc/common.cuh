@@ -6,6 +6,7 @@
 #include <cstdio>
 #include <cstdarg>
 #include <atomic>
+#include <vector>
 
 #include "../../include/b200trk.h"
 
@@ -42,6 +43,31 @@ extern std::atomic<uint64_t> g_launch_count;
 // Returns a device pointer with at least `bytes` bytes, 256-byte aligned; nullptr on failure (error set).
 void* workspace(size_t bytes, int slot = 0);
 int device_sm_count();
+
+// ---- what one library handle owns: device buffers, pinned host buffers and events, all released when the owner is destroyed ----
+// Each call returns 0, or sets the library error and returns non-zero like B200_CHECK_CUDA. The handle keeps plain pointers to what it
+// got as non-owning views. An owner that never allocated makes no CUDA call, so host-only handles stay usable without a device.
+class Owner {
+public:
+    Owner() = default;
+    Owner(const Owner&) = delete;
+    Owner& operator=(const Owner&) = delete;
+    ~Owner();
+
+    int alloc(void** p, size_t bytes, bool zero);                      // zero: cudaMemset the buffer to 0 after cudaMalloc
+    int upload(void** p, const void* host, size_t bytes);             // cudaMalloc + a copy of `bytes` from the host (no zero-fill)
+    int pinned(void** p, size_t bytes);                                // cudaMallocHost
+    int event(cudaEvent_t* ev, unsigned flags);
+    int release(void* p);                                              // frees one buffer of alloc / upload early (grow-only buffers)
+
+    template <class T> int alloc(T** p, size_t n, bool zero) { return alloc((void**)p, n * sizeof(T), zero); }
+    template <class T> int upload(T** p, const T* host, size_t n) { return upload((void**)p, (const void*)host, n * sizeof(T)); }
+    template <class T> int pinned(T** p, size_t n) { return pinned((void**)p, n * sizeof(T)); }
+
+private:
+    std::vector<void*> dev_, host_;
+    std::vector<cudaEvent_t> events_;
+};
 
 // ---- device helpers --------------------------------------------------------------------------------
 __device__ __forceinline__ float warp_sum(float v) {

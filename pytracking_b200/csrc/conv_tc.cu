@@ -518,9 +518,9 @@ static void pick_tile(int Wout, int Hout, int stride, int* BW, int* BH) {
     }
 }
 
-int tc_conv_prepare(b200trk_net* net, Op& op, const std::vector<float>& w_khwc) {
-    (void)w_khwc;                    // the repacked weights are read from op.w on the device
+int tc_conv_prepare(b200trk_net* net, Op& op) {
     TcConv* tc = new TcConv();
+    net->tcs.push_back(tc);
     op.tc = tc;
     TcParams& P = tc->P;
     memset(&P, 0, sizeof(P));
@@ -537,19 +537,12 @@ int tc_conv_prepare(b200trk_net* net, Op& op, const std::vector<float>& w_khwc) 
     P.residual = op.res >= 0 ? net->bufs[op.res] : nullptr;
     P.ws = net->splitk_ws;
     if (int e = make_map_4d(&P.a_map, net->bufs[op.in], op.Cin, op.Win, op.Hin, net->max_batch, P.BW, P.BH, op.stride)) return e;
-    void* cnt = nullptr;
-    B200_CHECK_CUDA(cudaMalloc(&cnt, 1024 * sizeof(unsigned)));
-    B200_CHECK_CUDA(cudaMemset(cnt, 0, 1024 * sizeof(unsigned)));
-    net->owned.push_back(cnt);
-    P.counters = (unsigned*)cnt;
+    if (int e = net->mem.alloc(&P.counters, 1024, true)) return e;
     // The B operand: the weights split into TF32 hi | lo (precision 2: rounded to TF32) once, here, instead of in every CTA that
     // loads them. op.w stays the raw fp32 weights (the plan's weight read-back and the exact-fp32 path use them).
     tc->single = net->precision == 2;
     const size_t nw = (size_t)op.Cout * op.k * op.k * op.Cin;
-    void* hl = nullptr;
-    B200_CHECK_CUDA(cudaMalloc(&hl, (tc->single ? 1 : 2) * nw * sizeof(float)));
-    net->owned.push_back(hl);
-    tc->w_split = (float*)hl;
+    if (int e = net->mem.alloc(&tc->w_split, (tc->single ? 1 : 2) * nw, false)) return e;
     const size_t blocks = (nw + 255) / 256;
     if (tc->single) tc_round_weights_kernel<<<(unsigned)(blocks < 4096 ? blocks : 4096), 256>>>(op.w, tc->w_split, nw);
     else tc_split_weights_kernel<<<(unsigned)(blocks < 4096 ? blocks : 4096), 256>>>(op.w, tc->w_split, nw);

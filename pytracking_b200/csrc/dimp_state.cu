@@ -8,13 +8,6 @@
 
 using namespace b200trk;
 
-static int st_alloc(b200trk_dimp_state* s, void** p, size_t bytes) {
-    B200_CHECK_CUDA(cudaMalloc(p, bytes));
-    B200_CHECK_CUDA(cudaMemset(*p, 0, bytes));
-    s->owned.push_back(*p);
-    return 0;
-}
-
 // The buffers both optimiser kinds share (and the GN LUTs when num_bins > 0); frees `s` on failure.  filter_ext: see dimp_state.cuh.
 static int state_alloc(b200trk_dimp_state* s, b200trk_net* net, int memory_size, int filter_size, const float* label_lut,
                        const float* mask_lut, const float* spatial_lut, int num_bins, float* filter_ext) {
@@ -25,19 +18,19 @@ static int state_alloc(b200trk_dimp_state* s, b200trk_net* net, int memory_size,
     const size_t plane = (size_t)s->Cc * s->Hc * s->Wc;
     int e = 0;
     if (filter_ext) s->filter = filter_ext;
-    else if (!e) e = st_alloc(s, (void**)&s->filter, (size_t)s->Cc * 16 * sizeof(float));
+    else if (!e) e = s->mem.alloc(&s->filter, (size_t)s->Cc * 16, true);
     s->mem_pitch = (s->Hc * s->Wc + 31) / 32 * 32;
-    if (!e) e = st_alloc(s, (void**)&s->memory, (size_t)s->Cc * s->mem_pitch * memory_size * sizeof(float));
-    if (!e) e = st_alloc(s, (void**)&s->boxes, (size_t)memory_size * 4 * sizeof(float));
-    if (!e) e = st_alloc(s, (void**)&s->sw, (size_t)memory_size * sizeof(float));
+    if (!e) e = s->mem.alloc(&s->memory, (size_t)s->Cc * s->mem_pitch * memory_size, true);
+    if (!e) e = s->mem.alloc(&s->boxes, (size_t)memory_size * 4, true);
+    if (!e) e = s->mem.alloc(&s->sw, (size_t)memory_size, true);
     if (!filter_ext) {
-        if (!e) e = st_alloc(s, (void**)&s->clf, plane * s->max_batch * sizeof(float));
-        if (!e) e = st_alloc(s, (void**)&s->scores, (size_t)s->max_batch * s->Ho * s->Wo * sizeof(float));
-        if (!e) e = st_alloc(s, (void**)&s->crop, (size_t)s->max_batch * 3 * net->crop_h * net->crop_w * sizeof(float));
-        if (!e) e = st_alloc(s, (void**)&s->maxval, (size_t)s->max_batch * sizeof(float));
-        if (!e) e = st_alloc(s, (void**)&s->maxidx, (size_t)s->max_batch * 2 * sizeof(int64_t));
+        if (!e) e = s->mem.alloc(&s->clf, plane * s->max_batch, true);
+        if (!e) e = s->mem.alloc(&s->scores, (size_t)s->max_batch * s->Ho * s->Wo, true);
+        if (!e) e = s->mem.alloc(&s->crop, (size_t)s->max_batch * 3 * net->crop_h * net->crop_w, true);
+        if (!e) e = s->mem.alloc(&s->maxval, (size_t)s->max_batch, true);
+        if (!e) e = s->mem.alloc(&s->maxidx, (size_t)s->max_batch * 2, true);
     }
-    if (!e && num_bins > 0) e = st_alloc(s, (void**)&s->luts, (size_t)3 * num_bins * sizeof(float));
+    if (!e && num_bins > 0) e = s->mem.alloc(&s->luts, (size_t)3 * num_bins, true);
     if (!e && num_bins > 0) {
         cudaError_t ce = cudaMemcpy(s->luts, label_lut, num_bins * sizeof(float), cudaMemcpyHostToDevice);
         if (ce == cudaSuccess) ce = cudaMemcpy(s->luts + num_bins, mask_lut, num_bins * sizeof(float), cudaMemcpyHostToDevice);
@@ -45,12 +38,10 @@ static int state_alloc(b200trk_dimp_state* s, b200trk_net* net, int memory_size,
         if (ce != cudaSuccess) { set_error("dimp_state_create: LUT upload failed: %s", cudaGetErrorString(ce)); e = 1; }
     }
     for (int i = 0; i < b200trk_dimp_state::NSTAGE && !e; ++i) {
-        if (cudaMallocHost((void**)&s->stage[i], (size_t)(4 + memory_size) * sizeof(float)) != cudaSuccess ||
-            cudaEventCreateWithFlags(&s->stage_ev[i], cudaEventDisableTiming) != cudaSuccess) {
-            set_error("dimp_state_create: pinned staging allocation failed"); e = 1;
-        }
+        e = s->mem.pinned(&s->stage[i], (size_t)4 + memory_size);
+        if (!e) e = s->mem.event(&s->stage_ev[i], cudaEventDisableTiming);
     }
-    if (e) b200trk_dimp_state_destroy(s);
+    if (e) delete s;
     return e;
 }
 
@@ -109,12 +100,6 @@ extern "C" int b200trk_prdimp_state_create(b200trk_dimp_state_t** out, b200trk_n
 extern "C" int b200trk_dimp_state_optimizer_kind(b200trk_dimp_state_t* s) { return s ? s->opt_kind : -1; }
 
 extern "C" int b200trk_dimp_state_destroy(b200trk_dimp_state_t* s) {
-    if (!s) return 0;
-    for (void* p : s->owned) cudaFree(p);
-    for (int i = 0; i < b200trk_dimp_state::NSTAGE; ++i) {
-        if (s->stage[i]) cudaFreeHost(s->stage[i]);
-        if (s->stage_ev[i]) cudaEventDestroy(s->stage_ev[i]);
-    }
     delete s;
     return 0;
 }

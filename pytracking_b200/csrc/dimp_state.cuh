@@ -5,6 +5,7 @@
 #include <vector>
 
 struct b200trk_dimp_state {
+    b200trk::Owner mem;     // the device buffers below (not `net`, nor a batch slot's filter), the staging ring and its events
     b200trk_net* net = nullptr;
     int memory_size = 0, ksz = 4, Cc = 0, Hc = 0, Wc = 0, Ho = 0, Wo = 0, num_bins = 0, max_batch = 1;
     int mem_pitch = 0;      // floats between two channel planes of the sample memory: H*W rounded up to 32, so that every 32-pixel
@@ -19,7 +20,6 @@ struct b200trk_dimp_state {
     float *filter = nullptr, *memory = nullptr, *boxes = nullptr, *sw = nullptr, *clf = nullptr, *scores = nullptr;
     float *crop = nullptr, *maxval = nullptr, *luts = nullptr;
     int64_t* maxidx = nullptr;
-    std::vector<void*> owned;
     // pinned staging ring for the small per-update H2D payload (box + sample weights): a slot is rewritten only after the copy
     // that read it has completed (its event), so back-to-back asynchronous update calls never race with their own uploads
     static constexpr int NSTAGE = 4;

@@ -72,6 +72,7 @@ struct FrameUpload {
 // host state
 // ---------------------------------------------------------------------------------------------------------------------------
 struct b200trk_dimp_tracker {
+    Owner mem;                                       // the device and pinned buffers below (not `st`, `iou_pred`, `mod_head`)
     b200trk_dimp_state* st = nullptr;
     b200trk_dimp_params_t p;
     // DiMP scalars (float32 tensors in the reference), [0] = row / height, [1] = column / width
@@ -208,11 +209,10 @@ extern "C" int b200trk_dimp_tracker_create(b200trk_dimp_tracker_t** out, b200trk
         t->kernel_size[0] = t->kernel_size[1] = (float)state->ksz;
         t->score_sz[0] = (float)state->Ho; t->score_sz[1] = (float)state->Wo;
         // a state without per-frame buffers is a batch slot: the batch holds the localisation results of all its slots
-        if (state->clf && (cudaMalloc((void**)&t->loc_dev, sizeof(b200trk_loc_result_t)) != cudaSuccess ||
-                           cudaMallocHost((void**)&t->loc_host, sizeof(b200trk_loc_result_t)) != cudaSuccess)) {
-            set_error("dimp_tracker_create: allocation failed");
-            b200trk_dimp_tracker_destroy(t);
-            return 1;
+        if (state->clf) {
+            int e = t->mem.alloc(&t->loc_dev, 1, false);
+            if (!e) e = t->mem.pinned(&t->loc_host, 1);
+            if (e) { delete t; return e; }
         }
     } else {
         t->feature_sz[0] = t->feature_sz[1] = (float)(params->image_sample_size / 16);
@@ -224,12 +224,6 @@ extern "C" int b200trk_dimp_tracker_create(b200trk_dimp_tracker_t** out, b200trk
 }
 
 extern "C" int b200trk_dimp_tracker_destroy(b200trk_dimp_tracker_t* t) {
-    if (!t) return 0;
-    if (t->loc_dev) cudaFree(t->loc_dev);
-    if (t->loc_host) cudaFreeHost(t->loc_host);
-    for (float* q : {t->mod3, t->mod4, t->iou3, t->iou4, t->boxes_dev, t->aug_mult, t->aug_patch}) if (q) cudaFree(q);
-    if (t->aug_table) cudaFree(t->aug_table);
-    if (t->boxes_host) cudaFreeHost(t->boxes_host);
     delete t;
     return 0;
 }
@@ -602,16 +596,16 @@ extern "C" int b200trk_dimp_tracker_attach_iounet(b200trk_dimp_tracker_t* t, b20
         B200_REQUIRE(md[0] == C3 && md[1] == C4, "dimp_tracker_attach_iounet: the modulation head gives %d / %d values, the IoU features have "
                      "%d / %d channels", md[0], md[1], C3, C4);
     }
-    B200_CHECK_CUDA(cudaMalloc((void**)&t->mod3, C3 * sizeof(float)));
-    B200_CHECK_CUDA(cudaMalloc((void**)&t->mod4, C4 * sizeof(float)));
+    if (int e = t->mem.alloc(&t->mod3, C3, false)) return e;
+    if (int e = t->mem.alloc(&t->mod4, C4, false)) return e;
     if (!native) {
         B200_CHECK_CUDA(cudaMemcpy(t->mod3, modulation3, C3 * sizeof(float), cudaMemcpyHostToDevice));
         B200_CHECK_CUDA(cudaMemcpy(t->mod4, modulation4, C4 * sizeof(float), cudaMemcpyHostToDevice));
     }
-    B200_CHECK_CUDA(cudaMalloc((void**)&t->iou3, (size_t)C3 * t->iou_dims[1] * t->iou_dims[2] * sizeof(float)));
-    B200_CHECK_CUDA(cudaMalloc((void**)&t->iou4, (size_t)C4 * t->iou_dims[4] * t->iou_dims[5] * sizeof(float)));
-    B200_CHECK_CUDA(cudaMalloc((void**)&t->boxes_dev, 16 * 5 * sizeof(float)));
-    B200_CHECK_CUDA(cudaMallocHost((void**)&t->boxes_host, 16 * 5 * sizeof(float)));
+    if (int e = t->mem.alloc(&t->iou3, (size_t)C3 * t->iou_dims[1] * t->iou_dims[2], false)) return e;
+    if (int e = t->mem.alloc(&t->iou4, (size_t)C4 * t->iou_dims[4] * t->iou_dims[5], false)) return e;
+    if (int e = t->mem.alloc(&t->boxes_dev, 16 * 5, false)) return e;
+    if (int e = t->mem.pinned(&t->boxes_host, 16 * 5)) return e;
     t->iou_pred = pred;
     t->mod_native = native ? 1 : 0;
     return 0;
@@ -733,12 +727,14 @@ extern "C" int b200trk_dimp_tracker_initialize_augmented_host(b200trk_dimp_track
     b200trk_crop_geom_t g; float boxes[4 * B200TRK_AUG_MAX];
     if (int e = b200trk_dimp_tracker_init_state_augmented(t, H, W, init_bbox, aug, &g, boxes)) return e;
     const size_t patch_floats = (size_t)3 * g.out_h * g.out_w, plane = (size_t)s->Cc * s->Hc * s->Wc;
-    if (!t->aug_table) B200_CHECK_CUDA(cudaMalloc(&t->aug_table, b200trk::augment_table_bytes()));
-    if (!t->aug_mult) B200_CHECK_CUDA(cudaMalloc((void**)&t->aug_mult, (size_t)B200TRK_AUG_MAX * s->Cc * sizeof(float)));
+    if (!t->aug_table)
+        if (int e = t->mem.alloc(&t->aug_table, b200trk::augment_table_bytes(), false)) return e;
+    if (!t->aug_mult)
+        if (int e = t->mem.alloc(&t->aug_mult, (size_t)B200TRK_AUG_MAX * s->Cc, false)) return e;
     if (patch_floats > t->aug_patch_cap) {
-        if (t->aug_patch) B200_CHECK_CUDA(cudaFree(t->aug_patch));
+        if (int e = t->mem.release(t->aug_patch)) return e;
         t->aug_patch = nullptr; t->aug_patch_cap = 0;
-        B200_CHECK_CUDA(cudaMalloc((void**)&t->aug_patch, patch_floats * sizeof(float)));
+        if (int e = t->mem.alloc(&t->aug_patch, patch_floats, false)) return e;
         t->aug_patch_cap = patch_floats;
     }
     if (int e = t->frames.upload(1, &image, &H, &W, st)) return e;
@@ -846,6 +842,7 @@ extern "C" int b200trk_dimp_track_device(b200trk_dimp_tracker_t* t, const uint8_
 // batch-mates, its slot or when they started -- and the network's cached graph (keyed on pointers and S) is replayed every step.
 // The online optimiser stays per sequence (dimp_state_insert / dimp_state_optimize on the slot's state), enqueued back to back.
 struct b200trk_dimp_batch {
+    Owner mem;                                                                       // the device and pinned buffers below
     b200trk_net* net = nullptr;
     int cap = 0, Cc = 0, Hc = 0, Wc = 0, Ho = 0, Wo = 0, ksz = 4, iss = 0;
     b200trk_dimp_params_t p;
@@ -864,8 +861,6 @@ extern "C" int b200trk_dimp_batch_destroy(b200trk_dimp_batch_t* b) {
         b200trk_dimp_tracker_destroy(t);
         b200trk_dimp_state_destroy(s);
     }
-    for (void* q : {(void*)b->crop, (void*)b->clf, (void*)b->scores, (void*)b->filters, (void*)b->loc_dev}) if (q) cudaFree(q);
-    if (b->loc_host) cudaFreeHost(b->loc_host);
     delete b;
     return 0;
 }
@@ -887,16 +882,13 @@ static int batch_create(b200trk_dimp_batch** out, b200trk_net* net, int capacity
     b->Ho = b->Hc + (filter_size + 1) % 2; b->Wo = b->Wc + (filter_size + 1) % 2;
     const size_t S = (size_t)capacity, fsz = (size_t)b->Cc * filter_size * filter_size;
     auto fail = [&](int e) { b200trk_dimp_batch_destroy(b); return e ? e : 1; };
-    auto alloc = [&](void** q, size_t bytes) {
-        return cudaMalloc(q, bytes) == cudaSuccess && cudaMemset(*q, 0, bytes) == cudaSuccess;
-    };
-    if (!alloc((void**)&b->crop, S * 3 * net->crop_h * net->crop_w * sizeof(float)) ||
-        !alloc((void**)&b->clf, S * b->Cc * b->Hc * b->Wc * sizeof(float)) || !alloc((void**)&b->scores, S * b->Ho * b->Wo * sizeof(float)) ||
-        !alloc((void**)&b->filters, S * fsz * sizeof(float)) || !alloc((void**)&b->loc_dev, S * sizeof(b200trk_loc_result_t)) ||
-        cudaMallocHost((void**)&b->loc_host, S * sizeof(b200trk_loc_result_t)) != cudaSuccess) {
-        set_error("dimp_batch_create: allocation failed");
-        return fail(1);
-    }
+    int e = b->mem.alloc(&b->crop, S * 3 * net->crop_h * net->crop_w, true);
+    if (!e) e = b->mem.alloc(&b->clf, S * b->Cc * b->Hc * b->Wc, true);
+    if (!e) e = b->mem.alloc(&b->scores, S * b->Ho * b->Wo, true);
+    if (!e) e = b->mem.alloc(&b->filters, S * fsz, true);
+    if (!e) e = b->mem.alloc(&b->loc_dev, S, true);
+    if (!e) e = b->mem.pinned(&b->loc_host, S);
+    if (e) return fail(e);
     for (int i = 0; i < capacity; ++i) {
         b200trk_dimp_state* s = nullptr;
         if (int e = make_state(b->filters + i * fsz, &s)) return fail(e);

@@ -91,7 +91,7 @@ struct b200trk_iou_modulation {
     int C3 = 0, C4 = 0, D = 0, M3 = 0, M4 = 0;       // c3_r / c4_r channels, fc3_1r outputs, fc34_3r / fc34_4r outputs
     float *w31 = nullptr, *b31 = nullptr, *w3 = nullptr, *b3 = nullptr, *w4 = nullptr, *b4 = nullptr;   // folded [out][in], [out]
     float *rois = nullptr, *pool3 = nullptr, *pool4 = nullptr, *cat = nullptr;                         // scratch for 16 boxes
-    std::vector<void*> owned;
+    Owner mem;
 };
 
 namespace {
@@ -110,14 +110,6 @@ void fold_block(const b200trk_linear_block_t& L, int out, int in, std::vector<fl
     }
 }
 
-int mod_alloc(b200trk_iou_modulation* m, float** q, size_t floats) {
-    void* d = nullptr;
-    B200_CHECK_CUDA(cudaMalloc(&d, floats * sizeof(float)));
-    m->owned.push_back(d);
-    *q = (float*)d;
-    return 0;
-}
-
 }  // namespace
 
 extern "C" int b200trk_iou_modulation_create(b200trk_iou_modulation_t** out, const b200trk_linear_block_t* fc3_1r,
@@ -130,30 +122,25 @@ extern "C" int b200trk_iou_modulation_create(b200trk_iou_modulation_t** out, con
     b200trk_iou_modulation* m = new b200trk_iou_modulation();
     m->C3 = C3; m->C4 = C4; m->D = D; m->M3 = M3; m->M4 = M4;
     std::vector<float> w, b;
-    int e = 0;
-    auto up = [&](float** dst, const std::vector<float>& v) {
-        if (e) return;
-        e = mod_alloc(m, dst, v.size());
-        if (!e && cudaMemcpy(*dst, v.data(), v.size() * sizeof(float), cudaMemcpyHostToDevice) != cudaSuccess) {
-            set_error("iou_modulation_create: upload failed");
-            e = 1;
-        }
-    };
-    fold_block(*fc3_1r, D, 9 * C3, w, b); up(&m->w31, w); up(&m->b31, b);
-    fold_block(*fc34_3r, M3, D + C4, w, b); up(&m->w3, w); up(&m->b3, b);
-    fold_block(*fc34_4r, M4, D + C4, w, b); up(&m->w4, w); up(&m->b4, b);
-    if (!e) e = mod_alloc(m, &m->rois, 5 * kFilterInitMax);
-    if (!e) e = mod_alloc(m, &m->pool3, (size_t)kFilterInitMax * 9 * C3);
-    if (!e) e = mod_alloc(m, &m->pool4, (size_t)kFilterInitMax * C4);
-    if (!e) e = mod_alloc(m, &m->cat, (size_t)kFilterInitMax * D);
-    if (e) { b200trk_iou_modulation_destroy(m); return e; }
+    fold_block(*fc3_1r, D, 9 * C3, w, b);
+    int e = m->mem.upload(&m->w31, w.data(), w.size());
+    if (!e) e = m->mem.upload(&m->b31, b.data(), b.size());
+    fold_block(*fc34_3r, M3, D + C4, w, b);
+    if (!e) e = m->mem.upload(&m->w3, w.data(), w.size());
+    if (!e) e = m->mem.upload(&m->b3, b.data(), b.size());
+    fold_block(*fc34_4r, M4, D + C4, w, b);
+    if (!e) e = m->mem.upload(&m->w4, w.data(), w.size());
+    if (!e) e = m->mem.upload(&m->b4, b.data(), b.size());
+    if (!e) e = m->mem.alloc(&m->rois, 5 * kFilterInitMax, false);
+    if (!e) e = m->mem.alloc(&m->pool3, (size_t)kFilterInitMax * 9 * C3, false);
+    if (!e) e = m->mem.alloc(&m->pool4, (size_t)kFilterInitMax * C4, false);
+    if (!e) e = m->mem.alloc(&m->cat, (size_t)kFilterInitMax * D, false);
+    if (e) { delete m; return e; }
     *out = m;
     return 0;
 }
 
 extern "C" int b200trk_iou_modulation_destroy(b200trk_iou_modulation_t* m) {
-    if (!m) return 0;
-    for (void* q : m->owned) cudaFree(q);
     delete m;
     return 0;
 }

@@ -22,22 +22,10 @@ struct b200trk_iou_predictor {
     // per-call scratch (R <= RMAX)
     float *rois = nullptr, *pool3 = nullptr, *pool4 = nullptr, *act = nullptr, *gpool3 = nullptr, *gpool4 = nullptr;
     float *grois3 = nullptr, *grois4 = nullptr, *rel = nullptr, *sznorm = nullptr, *step = nullptr, *part = nullptr;
-    std::vector<void*> owned;
+    Owner mem;
 };
 
 #include "iou_refine_kernels.cuh"      // IOU_RMAX, FC_KS, the seven kernels, fold_linear (anonymous namespace)
-
-namespace {
-
-int iou_alloc(b200trk_iou_predictor* p, float** q, size_t floats) {
-    void* d = nullptr;
-    B200_CHECK_CUDA(cudaMalloc(&d, floats * sizeof(float)));
-    p->owned.push_back(d);
-    *q = (float*)d;
-    return 0;
-}
-
-}  // namespace
 
 extern "C" int b200trk_iou_predictor_create(b200trk_iou_predictor_t** out, const b200trk_linear_block_t* fc3_rt, const b200trk_linear_block_t* fc4_rt,
                                             const float* iou_predictor_weight, const float* iou_predictor_bias, int C3, int P3, int C4, int P4,
@@ -48,37 +36,32 @@ extern "C" int b200trk_iou_predictor_create(b200trk_iou_predictor_t** out, const
     p->C3 = C3; p->P3 = P3; p->C4 = C4; p->P4 = P4; p->D3 = D3; p->D4 = D4;
     const int K3 = C3 * P3 * P3, K4 = C4 * P4 * P4;
     std::vector<float> w, b;
-    int e = 0;
-    auto up = [&](float** dst, const std::vector<float>& v) {
-        if (e) return;
-        e = iou_alloc(p, dst, v.size());
-        if (!e && cudaMemcpy(*dst, v.data(), v.size() * sizeof(float), cudaMemcpyHostToDevice) != cudaSuccess) { set_error("iou_predictor_create: upload failed"); e = 1; }
-    };
-    fold_linear(*fc3_rt, D3, K3, w, b); up(&p->w3, w); up(&p->b3, b);
-    fold_linear(*fc4_rt, D4, K4, w, b); up(&p->w4, w); up(&p->b4, b);
-    std::vector<float> wp(iou_predictor_weight, iou_predictor_weight + D3 + D4);
-    up(&p->wp, wp);
+    fold_linear(*fc3_rt, D3, K3, w, b);
+    int e = p->mem.upload(&p->w3, w.data(), w.size());
+    if (!e) e = p->mem.upload(&p->b3, b.data(), b.size());
+    fold_linear(*fc4_rt, D4, K4, w, b);
+    if (!e) e = p->mem.upload(&p->w4, w.data(), w.size());
+    if (!e) e = p->mem.upload(&p->b4, b.data(), b.size());
+    if (!e) e = p->mem.upload(&p->wp, iou_predictor_weight, (size_t)D3 + D4);
     p->bp = iou_predictor_bias ? iou_predictor_bias[0] : 0.f;
-    if (!e) e = iou_alloc(p, &p->rois, IOU_RMAX * 5);
-    if (!e) e = iou_alloc(p, &p->pool3, (size_t)IOU_RMAX * K3);
-    if (!e) e = iou_alloc(p, &p->pool4, (size_t)IOU_RMAX * K4);
-    if (!e) e = iou_alloc(p, &p->gpool3, (size_t)IOU_RMAX * K3);
-    if (!e) e = iou_alloc(p, &p->gpool4, (size_t)IOU_RMAX * K4);
-    if (!e) e = iou_alloc(p, &p->act, (size_t)IOU_RMAX * (D3 + D4));
-    if (!e) e = iou_alloc(p, &p->part, (size_t)((K3 > K4 ? K3 : K4) / FC_KS + 1) * IOU_RMAX * (D3 + D4));
-    if (!e) e = iou_alloc(p, &p->grois3, IOU_RMAX * 5);
-    if (!e) e = iou_alloc(p, &p->grois4, IOU_RMAX * 5);
-    if (!e) e = iou_alloc(p, &p->rel, IOU_RMAX * 4);
-    if (!e) e = iou_alloc(p, &p->sznorm, 4);
-    if (!e) e = iou_alloc(p, &p->step, 4);
-    if (e) { b200trk_iou_predictor_destroy(p); return e; }
+    if (!e) e = p->mem.alloc(&p->rois, IOU_RMAX * 5, false);
+    if (!e) e = p->mem.alloc(&p->pool3, (size_t)IOU_RMAX * K3, false);
+    if (!e) e = p->mem.alloc(&p->pool4, (size_t)IOU_RMAX * K4, false);
+    if (!e) e = p->mem.alloc(&p->gpool3, (size_t)IOU_RMAX * K3, false);
+    if (!e) e = p->mem.alloc(&p->gpool4, (size_t)IOU_RMAX * K4, false);
+    if (!e) e = p->mem.alloc(&p->act, (size_t)IOU_RMAX * (D3 + D4), false);
+    if (!e) e = p->mem.alloc(&p->part, (size_t)((K3 > K4 ? K3 : K4) / FC_KS + 1) * IOU_RMAX * (D3 + D4), false);
+    if (!e) e = p->mem.alloc(&p->grois3, IOU_RMAX * 5, false);
+    if (!e) e = p->mem.alloc(&p->grois4, IOU_RMAX * 5, false);
+    if (!e) e = p->mem.alloc(&p->rel, IOU_RMAX * 4, false);
+    if (!e) e = p->mem.alloc(&p->sznorm, 4, false);
+    if (!e) e = p->mem.alloc(&p->step, 4, false);
+    if (e) { delete p; return e; }
     *out = p;
     return 0;
 }
 
 extern "C" int b200trk_iou_predictor_destroy(b200trk_iou_predictor_t* p) {
-    if (!p) return 0;
-    for (void* q : p->owned) cudaFree(q);
     delete p;
     return 0;
 }

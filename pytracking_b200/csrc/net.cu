@@ -5,29 +5,16 @@
 #include <cmath>
 #include <cstring>
 
-namespace b200trk {
-
-int tc_conv_prepare(b200trk_net* net, Op& op, const std::vector<float>& w_khwc);   // conv_tc.cu
-int tc_conv_launch(b200trk_net* net, const Op& op, int S, cudaStream_t st);         // conv_tc.cu
-void tc_conv_free(TcConv* tc);
-bool tc_conv_supported(const Op& op);
-
-static int dev_alloc(b200trk_net* net, float** p, size_t floats) {
-    void* q = nullptr;
-    B200_CHECK_CUDA(cudaMalloc(&q, floats * sizeof(float)));
-    net->owned.push_back(q);
-    *p = (float*)q;
-    return 0;
-}
-
-static int new_buf(b200trk_net* net, size_t floats_per_sample, int* id) {
+int b200trk_net::add_buf(size_t floats_per_sample, int* id, bool zero) {
     float* p = nullptr;
-    if (int e = dev_alloc(net, &p, floats_per_sample * (size_t)net->max_batch)) return e;
-    net->bufs.push_back(p);
-    net->buf_floats.push_back(floats_per_sample);
-    *id = (int)net->bufs.size() - 1;
+    if (int e = mem.alloc(&p, floats_per_sample * (size_t)max_batch, zero)) return e;
+    bufs.push_back(p);
+    buf_floats.push_back(floats_per_sample);
+    *id = (int)bufs.size() - 1;
     return 0;
 }
+
+namespace b200trk {
 
 // fold eval-mode BN into (w, b) in double precision; repack [cout][cin][k][k] -> [cout][k][k][cin]
 static void fold_and_repack(const b200trk_conv_desc_t& d, std::vector<float>& w_out, std::vector<float>& b_out, bool& has_bias) {
@@ -49,43 +36,33 @@ static void fold_and_repack(const b200trk_conv_desc_t& d, std::vector<float>& w_
     }
 }
 
-struct Builder {
-    b200trk_net* net;
-    const b200trk_conv_desc_t* convs;
-    int n_convs, next = 0;
-
-    int add_conv(int in, int res, int Hin, int Win, int cin, int cout, int k, int stride, int pad, int relu, int* out_id,
-                 int* Hout_, int* Wout_) {
-        B200_REQUIRE(next < n_convs, "net_create: ran out of conv descriptors at #%d", next);
-        const b200trk_conv_desc_t& d = convs[next];
-        B200_REQUIRE(d.cin == cin && d.cout == cout && d.k == k && d.stride == stride && d.pad == pad && d.weight,
-                     "net_create: conv #%d is (cin=%d,cout=%d,k=%d,s=%d,p=%d) but the architecture expects (%d,%d,%d,%d,%d)",
-                     next, d.cin, d.cout, d.k, d.stride, d.pad, cin, cout, k, stride, pad);
-        ++next;
-        Op op;
-        op.kind = OP_CONV;
-        op.in = in; op.res = res;
-        op.Hin = Hin; op.Win = Win; op.Cin = cin; op.Cout = cout; op.k = k; op.stride = stride; op.pad = pad; op.relu = relu;
-        op.Hout = (Hin + 2 * pad - k) / stride + 1;
-        op.Wout = (Win + 2 * pad - k) / stride + 1;
-        std::vector<float> w, b; bool hb;
-        fold_and_repack(d, w, b, hb);
-        if (int e = dev_alloc(net, &op.w, w.size())) return e;
-        B200_CHECK_CUDA(cudaMemcpy(op.w, w.data(), w.size() * sizeof(float), cudaMemcpyHostToDevice));
-        if (hb) {
-            if (int e = dev_alloc(net, &op.bias, b.size())) return e;
-            B200_CHECK_CUDA(cudaMemcpy(op.bias, b.data(), b.size() * sizeof(float), cudaMemcpyHostToDevice));
-        }
-        if (int e = new_buf(net, (size_t)op.Hout * op.Wout * cout, &op.out)) return e;
-        if (net->precision != 1 && tc_conv_supported(op)) {
-            if (int e = tc_conv_prepare(net, op, w)) return e;
-        }
-        net->flops += 2.0 * (double)op.Hout * op.Wout * cout * (double)k * k * cin;
-        net->ops.push_back(op);
-        *out_id = op.out; *Hout_ = op.Hout; *Wout_ = op.Wout;
-        return 0;
-    }
-};
+int Builder::add_conv(int in, int res, int Hin, int Win, int cin, int cout, int k, int stride, int pad, int relu, int* out_id, int* Hout_,
+                      int* Wout_) {
+    B200_REQUIRE(next < n_convs, "net_create: ran out of conv descriptors at #%d", next);
+    const b200trk_conv_desc_t& d = convs[next];
+    B200_REQUIRE(d.cin == cin && d.cout == cout && d.k == k && d.stride == stride && d.pad == pad && d.weight,
+                 "net_create: conv #%d is (cin=%d,cout=%d,k=%d,s=%d,p=%d) but the architecture expects (%d,%d,%d,%d,%d)",
+                 next, d.cin, d.cout, d.k, d.stride, d.pad, cin, cout, k, stride, pad);
+    ++next;
+    Op op;
+    op.kind = OP_CONV;
+    op.in = in; op.res = res;
+    op.Hin = Hin; op.Win = Win; op.Cin = cin; op.Cout = cout; op.k = k; op.stride = stride; op.pad = pad; op.relu = relu;
+    op.Hout = (Hin + 2 * pad - k) / stride + 1;
+    op.Wout = (Win + 2 * pad - k) / stride + 1;
+    std::vector<float> w, b; bool hb;
+    fold_and_repack(d, w, b, hb);
+    if (int e = net->mem.upload(&op.w, w.data(), w.size())) return e;
+    if (hb)
+        if (int e = net->mem.upload(&op.bias, b.data(), b.size())) return e;
+    if (int e = net->add_buf((size_t)op.Hout * op.Wout * cout, &op.out)) return e;
+    if (net->precision != 1 && tc_conv_supported(op))
+        if (int e = tc_conv_prepare(net, op)) return e;
+    net->flops += 2.0 * (double)op.Hout * op.Wout * cout * (double)k * k * cin;
+    net->ops.push_back(op);
+    *out_id = op.out; *Hout_ = op.Hout; *Wout_ = op.Wout;
+    return 0;
+}
 
 static int build(b200trk_net* net, const b200trk_conv_desc_t* convs, int n_convs) {
     Builder B{net, convs, n_convs};
@@ -99,7 +76,7 @@ static int build(b200trk_net* net, const b200trk_conv_desc_t* convs, int n_convs
     int H = net->crop_h, W = net->crop_w;
     // preprocess -> NHWC4
     int b_in;
-    if (int e = new_buf(net, (size_t)H * W * 4, &b_in)) return e;
+    if (int e = net->add_buf((size_t)H * W * 4, &b_in)) return e;
     { Op op; op.kind = OP_PREPROCESS; op.out = b_in; op.Hin = H; op.Win = W; net->ops.push_back(op); }
     // stem
     {
@@ -115,11 +92,9 @@ static int build(b200trk_net* net, const b200trk_conv_desc_t* convs, int n_convs
                 for (int ci = 0; ci < 3; ++ci) w4[((size_t)t * 3 + ci) * 64 + co] = w[((size_t)co * 49 + t) * 3 + ci];
         Op op; op.kind = OP_STEM; op.in = b_in; op.Hin = H; op.Win = W; op.Cin = 3; op.Cout = 64; op.k = 7; op.stride = 2; op.pad = 3;
         op.Hout = (H + 6 - 7) / 2 + 1; op.Wout = (W + 6 - 7) / 2 + 1; op.relu = 1;
-        if (int e = dev_alloc(net, &op.w, w4.size())) return e;
-        B200_CHECK_CUDA(cudaMemcpy(op.w, w4.data(), w4.size() * sizeof(float), cudaMemcpyHostToDevice));
-        if (int e = dev_alloc(net, &op.bias, 64)) return e;
-        B200_CHECK_CUDA(cudaMemcpy(op.bias, b.data(), 64 * sizeof(float), cudaMemcpyHostToDevice));
-        if (int e = new_buf(net, (size_t)op.Hout * op.Wout * 64, &op.out)) return e;
+        if (int e = net->mem.upload(&op.w, w4.data(), w4.size())) return e;
+        if (int e = net->mem.upload(&op.bias, b.data(), 64)) return e;
+        if (int e = net->add_buf((size_t)op.Hout * op.Wout * 64, &op.out)) return e;
         net->flops += 2.0 * (double)op.Hout * op.Wout * 64 * 49 * 3;
         net->ops.push_back(op);
         H = op.Hout; W = op.Wout;
@@ -129,7 +104,7 @@ static int build(b200trk_net* net, const b200trk_conv_desc_t* convs, int n_convs
     {
         Op op; op.kind = OP_MAXPOOL; op.in = x; op.Hin = H; op.Win = W; op.Cin = op.Cout = 64;
         op.Hout = (H + 2 - 3) / 2 + 1; op.Wout = (W + 2 - 3) / 2 + 1;
-        if (int e = new_buf(net, (size_t)op.Hout * op.Wout * 64, &op.out)) return e;
+        if (int e = net->add_buf((size_t)op.Hout * op.Wout * 64, &op.out)) return e;
         net->ops.push_back(op);
         H = op.Hout; W = op.Wout; x = op.out;
     }
@@ -203,20 +178,21 @@ extern "C" int b200trk_net_create(b200trk_net_t** out, int arch, const b200trk_c
     net->norm_scale = norm_scale;
     net->sms = device_sm_count();
     net->splitk_ws_floats = (size_t)8 << 20;   // 32 MB of split-K partials
-    int e = dev_alloc(net, &net->splitk_ws, net->splitk_ws_floats);
+    int e = net->mem.alloc(&net->splitk_ws, net->splitk_ws_floats, false);
     if (!e) e = build(net, convs, n_convs);
-    if (!e) e = dev_alloc(net, &net->l2_partials, 64 * 64);
-    if (e) { b200trk_net_destroy(net); return e; }
+    if (!e) e = net->mem.alloc(&net->l2_partials, 64 * 64, false);
+    if (e) { delete net; return e; }
     *out = net;
     return 0;
 }
 
+b200trk_net::~b200trk_net() {
+    drop_graph(this);
+    if (cap_stream) cudaStreamDestroy(cap_stream);
+    for (TcConv* tc : tcs) tc_conv_free(tc);
+}
+
 extern "C" int b200trk_net_destroy(b200trk_net_t* net) {
-    if (!net) return 0;
-    drop_graph(net);
-    if (net->cap_stream) cudaStreamDestroy(net->cap_stream);
-    for (auto& op : net->ops) if (op.tc) tc_conv_free(op.tc);
-    for (void* p : net->owned) cudaFree(p);
     delete net;
     return 0;
 }
@@ -225,10 +201,6 @@ extern "C" int b200trk_net_dims(const b200trk_net_t* net, int dims[9]) {
     B200_REQUIRE(net && dims, "net_dims: null pointer");
     memcpy(dims, net->dims, sizeof(int) * 9);
     return 0;
-}
-
-namespace b200trk {
-int tc_conv_set_debug(Op& op, unsigned long long* buf); int tc_conv_grid(const Op& op, int dims[4]); int tc_conv_reduction(const Op& op);
 }
 
 // Debug: attach (or detach, buf = NULL) a device buffer of [ctas][8] u64 phase time stamps to plan step `index`.
@@ -318,6 +290,14 @@ extern "C" int b200trk_net_attach_iou_head(b200trk_net_t* net, const b200trk_con
     B200_REQUIRE(net && convs, "net_attach_iou_head: null pointer");
     B200_REQUIRE(net->iou_dims[0] == 0, "net_attach_iou_head: already attached");
     B200_REQUIRE(net->feat_buf[0] >= 0 && net->feat_buf[1] >= 0, "net_attach_iou_head: the network has no layer2 / layer3 outputs");
+    // every refusal before the plan changes
+    for (int i = 0; i < 4; ++i) {
+        const b200trk_conv_desc_t& d = convs[i];
+        const int cin = i % 2 == 0 ? net->feat_hw[i / 2][0] : convs[i - 1].cout;
+        B200_REQUIRE(d.weight && d.cin == cin && d.cout > 0 && d.k == 3 && d.stride == 1 && d.pad == 1,
+                     "net_attach_iou_head: conv%d_%dt is (cin=%d,cout=%d,k=%d,s=%d,p=%d), the head needs (%d,cout,3,1,1)", 3 + i / 2, 1 + i % 2,
+                     d.cin, d.cout, d.k, d.stride, d.pad, cin);
+    }
     drop_graph(net);
     Builder B{net, convs, 4};
     const size_t first = net->ops.size();
@@ -334,8 +314,7 @@ extern "C" int b200trk_net_attach_iou_head(b200trk_net_t* net, const b200trk_con
     return 0;
 }
 
-// One convolution step of the plan at batch S: the tensor-core kernel where the step has one, else the fp32 CUDA-core kernel.
-static int conv_step(b200trk_net_t* net, const Op& op, int S, cudaStream_t st) {
+int b200trk::conv_step(b200trk_net* net, const Op& op, int S, cudaStream_t st) {
     if (op.tc) return tc_conv_launch(net, op, S, st);
     ConvShape sh{S, op.Hin, op.Win, op.Cin, op.Hout, op.Wout, op.Cout, op.k, op.stride, op.pad};
     ConvEpilogue ep{op.bias, op.res >= 0 ? net->bufs[op.res] : nullptr, op.relu};
@@ -363,7 +342,7 @@ extern "C" int b200trk_net_attach_filter_init(b200trk_net_t* net, const b200trk_
     const double flops = net->flops;
     Op imp; imp.kind = OP_NCHW_IMPORT; imp.init = 1;
     imp.Hin = imp.Hout = H; imp.Win = imp.Wout = W; imp.Cin = imp.Cout = C;
-    if (int e = new_buf(net, (size_t)H * W * C, &imp.out)) return e;
+    if (int e = net->add_buf((size_t)H * W * C, &imp.out)) return e;
     net->ops.push_back(imp);
     Builder B{net, conv, 1};
     int o, h, w;
@@ -372,9 +351,9 @@ extern "C" int b200trk_net_attach_filter_init(b200trk_net_t* net, const b200trk_
     auto& f = net->finit;
     f.import_op = (int)net->ops.size() - 2; f.conv_op = (int)net->ops.size() - 1;
     f.ksz = filter_size; f.norm = filter_norm != 0; f.square = pool_square != 0;
-    if (int e = new_buf(net, (size_t)H * W * C, &f.nchw)) return e;
-    if (int e = dev_alloc(net, &f.rois, 5 * 16)) return e;
-    if (int e = dev_alloc(net, &f.pooled, (size_t)16 * C * filter_size * filter_size)) return e;
+    if (int e = net->add_buf((size_t)H * W * C, &f.nchw)) return e;
+    if (int e = net->mem.alloc(&f.rois, 5 * 16, false)) return e;
+    if (int e = net->mem.alloc(&f.pooled, (size_t)16 * C * filter_size * filter_size, false)) return e;
     net->flops = flops;
     return 0;
 }
@@ -402,7 +381,7 @@ extern "C" int b200trk_net_attach_iou_ref(b200trk_net_t* net, const b200trk_conv
         if (int e = B.add_conv(net->feat_buf[lvl], -1, H, W, C, convs[lvl].cout, 3, 1, 1, 1, &o, &h, &w)) return e;
         net->ops.back().init = 1;
         f.op[lvl] = (int)net->ops.size() - 1;
-        if (int e = new_buf(net, (size_t)h * w * convs[lvl].cout, &f.nchw[lvl])) return e;
+        if (int e = net->add_buf((size_t)h * w * convs[lvl].cout, &f.nchw[lvl])) return e;
         f.dims[3 * lvl] = convs[lvl].cout; f.dims[3 * lvl + 1] = h; f.dims[3 * lvl + 2] = w;
     }
     net->flops = flops;

@@ -20,7 +20,7 @@ struct Op {
     int export_slot = -1;    // OP_EXPORT_NCHW: 0 = layer2, 1 = layer3, 2 / 3 = the IoUNet features of layer2 / layer3
     int iou = 0;             // belongs to the IoUNet feature branch (skipped when no IoU output is requested)
     int init = 0;            // belongs to a first-frame head (run by filter_init_conv / iou_ref_conv only, never by a forward pass)
-    TcConv* tc = nullptr;
+    TcConv* tc = nullptr;    // owned by the plan (b200trk_net::tcs)
 };
 
 }  // namespace b200trk
@@ -29,6 +29,32 @@ struct b200trk_net;
 struct b200trk_iou_modulation;
 
 namespace b200trk {
+// The tensor-core convolution of a plan step (conv_tc.cu).  tc_conv_prepare gives `op` a TcConv that `net` owns from then on, also when
+// it fails later; the weights are read from op.w on the device.  The debug calls report or instrument the launch as last configured.
+bool tc_conv_supported(const Op& op);
+int tc_conv_prepare(b200trk_net* net, Op& op);
+int tc_conv_launch(b200trk_net* net, const Op& op, int S, cudaStream_t st);
+void tc_conv_free(TcConv* tc);
+int tc_conv_set_debug(Op& op, unsigned long long* buf);
+int tc_conv_grid(const Op& op, int dims[4]);
+int tc_conv_tile(const Op& op, int dims[2]);
+int tc_conv_reduction(const Op& op);
+
+// One convolution step of the plan at batch S: the tensor-core kernel where the step has one, else the fp32 CUDA-core kernel (net.cu).
+int conv_step(b200trk_net* net, const Op& op, int S, cudaStream_t st);
+
+// Appends convolution steps to a plan from state_dict descriptors, consumed in order: BN folded in double, weights repacked OIHW -> OHWI
+// and uploaded with the bias, an output buffer added, the tensor-core path prepared unless the plan's precision is 1 or the shape is
+// unsupported, and the FLOPs counted (net.cu).
+struct Builder {
+    b200trk_net* net;
+    const b200trk_conv_desc_t* convs;
+    int n_convs, next = 0;
+
+    int add_conv(int in, int res, int Hin, int Win, int cin, int cout, int k, int stride, int pad, int relu, int* out_id, int* Hout_,
+                 int* Wout_);
+};
+
 // FilterInitializerLinear in two halves, so that a batch runs filter_conv once for all its images and pools each sequence's box apart:
 // filter_conv on the S normalised classification feature maps clf [S,C,H,W] (net.cu), then PrRoIPool of box r [x,y,w,h] on image
 // images[r] and the mean over the n boxes into filter [1,C,k,k] (init_heads.cu).
@@ -52,12 +78,13 @@ int feature_dropout(float* clf, int T, int num, int C, int HW, const float* mult
 }  // namespace b200trk
 
 struct b200trk_net {
+    b200trk::Owner mem;                  // every device allocation of the plan
+    std::vector<b200trk::TcConv*> tcs;   // every TcConv tc_conv_prepare made for the plan
     int arch = 0, crop_h = 0, crop_w = 0, max_batch = 0, precision = 0;
     float norm_scale = 1.f;
     std::vector<b200trk::Op> ops;
     std::vector<float*> bufs;            // activation buffers (device, NHWC fp32), sized for max_batch
     std::vector<size_t> buf_floats;      // per-sample floats of each buffer
-    std::vector<void*> owned;            // every device allocation (freed in destroy)
     float* splitk_ws = nullptr; size_t splitk_ws_floats = 0;
     float* l2_partials = nullptr;
     int dims[9] = {0};
@@ -75,4 +102,8 @@ struct b200trk_net {
     cudaGraphExec_t gexec = nullptr;
     uint64_t graph_kernels = 0;
     cudaStream_t cap_stream = nullptr;
+
+    // a new activation buffer of max_batch x floats_per_sample floats (zero: filled with 0) -> its id
+    int add_buf(size_t floats_per_sample, int* id, bool zero = false);
+    ~b200trk_net();                      // drops the cached graph and the capture stream, frees the TcConvs, then the memory
 };

@@ -9,14 +9,6 @@
 #include <cmath>
 #include <cstring>
 
-namespace b200trk {
-
-int tc_conv_prepare(b200trk_net* net, Op& op, const std::vector<float>& w_khwc);
-int tc_conv_launch(b200trk_net* net, const Op& op, int S, cudaStream_t st);
-bool tc_conv_supported(const Op& op);
-
-}  // namespace b200trk
-
 #include "tower_kernels.cuh"      // import_scaled, groupnorm1_relu, export_exp
 
 using namespace b200trk;
@@ -28,79 +20,43 @@ struct b200trk_tower {
     int stop_after = -1;         // debug: forward returns after this launch of its fixed sequence (-1: runs to the end)
 };
 
-extern "C" int b200trk_tower_destroy(b200trk_tower_t* t);
-
-static int tower_alloc(b200trk_net* net, float** p, size_t floats) {
-    void* q = nullptr;
-    B200_CHECK_CUDA(cudaMalloc(&q, floats * sizeof(float)));
-    net->owned.push_back(q);
-    *p = (float*)q;
-    return 0;
-}
-
 extern "C" int b200trk_tower_create(b200trk_tower_t** out, const b200trk_conv_desc_t* convs, int n_convs, const float* const* gn_gamma,
                                     const float* const* gn_beta, int C, int H, int W, int max_batch, int precision) {
     B200_REQUIRE(out && convs && gn_gamma && gn_beta, "tower_create: null pointer");
     B200_REQUIRE(n_convs >= 2 && n_convs <= 9 && C % 32 == 0 && H > 0 && W > 0 && max_batch >= 1 && max_batch <= 16, "tower_create: bad shape");
     B200_REQUIRE(precision >= 0 && precision <= 2,
                  "tower_create: precision %d must be 0 (3xTF32 tensor cores), 1 (fp32 CUDA cores) or 2 (TF32 tensor cores)", precision);
+    // every refusal before anything is allocated; a BatchNorm would be folded by the plan builder, but the tower has none
+    for (int i = 0, cin = C; i < n_convs; ++i) {
+        const b200trk_conv_desc_t& d = convs[i];
+        B200_REQUIRE(d.cin == cin && d.k == 3 && d.stride == 1 && d.pad == 1 && d.weight && !d.bn_gamma,
+                     "tower_create: conv #%d must be 3x3 / stride 1 / pad 1 with %d input channels and no BatchNorm", i, cin);
+        cin = d.cout;
+    }
     b200trk_tower* t = new b200trk_tower();
     b200trk_net* net = &t->net;
     net->max_batch = max_batch; net->precision = precision; net->crop_h = H; net->crop_w = W; net->sms = device_sm_count();
     net->splitk_ws_floats = (size_t)2 << 20;
     t->C = C; t->H = H; t->W = W;
-    int e = tower_alloc(net, &net->splitk_ws, net->splitk_ws_floats);
-    float* inb = nullptr;
-    if (!e) e = tower_alloc(net, &inb, (size_t)max_batch * H * W * C);
-    if (!e) { net->bufs.push_back(inb); net->buf_floats.push_back((size_t)H * W * C); t->in_buf = 0; }
-    int x = 0, cin = C;
-    for (int i = 0; i < n_convs && !e; ++i) {
-        const b200trk_conv_desc_t& d = convs[i];
-        if (!(d.cin == cin && d.k == 3 && d.stride == 1 && d.pad == 1 && d.weight && !d.bn_gamma)) {
-            set_error("tower_create: conv #%d must be 3x3 / stride 1 / pad 1 with %d input channels and no BatchNorm", i, cin);
-            e = 2; break;
-        }
-        Op op; op.kind = OP_CONV; op.in = x; op.res = -1;
-        op.Hin = op.Hout = H; op.Win = op.Wout = W; op.Cin = cin; op.Cout = d.cout; op.k = 3; op.stride = 1; op.pad = 1; op.relu = 0;
-        std::vector<float> w((size_t)d.cout * 9 * d.cin);
-        for (int co = 0; co < d.cout; ++co)
-            for (int ci = 0; ci < d.cin; ++ci)
-                for (int tt = 0; tt < 9; ++tt) w[((size_t)co * 9 + tt) * d.cin + ci] = d.weight[((size_t)co * d.cin + ci) * 9 + tt];
-        e = tower_alloc(net, &op.w, w.size());
-        if (!e && cudaMemcpy(op.w, w.data(), w.size() * sizeof(float), cudaMemcpyHostToDevice) != cudaSuccess) { set_error("tower_create: upload failed"); e = 1; }
-        if (!e && d.bias) {
-            e = tower_alloc(net, &op.bias, d.cout);
-            if (!e && cudaMemcpy(op.bias, d.bias, d.cout * sizeof(float), cudaMemcpyHostToDevice) != cudaSuccess) { set_error("tower_create: upload failed"); e = 1; }
-        }
-        float* ob = nullptr;
-        if (!e) e = tower_alloc(net, &ob, (size_t)max_batch * H * W * d.cout);
-        if (!e) { net->bufs.push_back(ob); net->buf_floats.push_back((size_t)H * W * d.cout); op.out = (int)net->bufs.size() - 1; }
-        if (!e && precision != 1 && tc_conv_supported(op)) e = tc_conv_prepare(net, op, w);
-        if (!e) {
-            net->flops += 2.0 * H * W * (double)d.cout * 9.0 * d.cin;
-            net->ops.push_back(op);
-            x = op.out; cin = d.cout;
-            if (i < n_convs - 1) {
-                float *g = nullptr, *b = nullptr;
-                e = tower_alloc(net, &g, d.cout);
-                if (!e) e = tower_alloc(net, &b, d.cout);
-                if (!e && (cudaMemcpy(g, gn_gamma[i], d.cout * sizeof(float), cudaMemcpyHostToDevice) != cudaSuccess ||
-                           cudaMemcpy(b, gn_beta[i], d.cout * sizeof(float), cudaMemcpyHostToDevice) != cudaSuccess)) { set_error("tower_create: upload failed"); e = 1; }
-                t->gamma.push_back(g); t->beta.push_back(b);
-            }
+    int e = net->mem.alloc(&net->splitk_ws, net->splitk_ws_floats, false);
+    if (!e) e = net->add_buf((size_t)H * W * C, &t->in_buf);
+    Builder B{net, convs, n_convs};
+    for (int i = 0, x = t->in_buf, h, w; i < n_convs && !e; ++i) {
+        const int cin = convs[i].cin, cout = convs[i].cout;
+        e = B.add_conv(x, -1, H, W, cin, cout, 3, 1, 1, 0, &x, &h, &w);
+        if (!e && i < n_convs - 1) {
+            float *g = nullptr, *b = nullptr;
+            e = net->mem.upload(&g, gn_gamma[i], cout);
+            if (!e) e = net->mem.upload(&b, gn_beta[i], cout);
+            t->gamma.push_back(g); t->beta.push_back(b);
         }
     }
-    if (e) { b200trk_tower_destroy(t); return e; }
+    if (e) { delete t; return e; }
     *out = t;
     return 0;
 }
 
-namespace b200trk { void tc_conv_free(TcConv* tc); }
-
 extern "C" int b200trk_tower_destroy(b200trk_tower_t* t) {
-    if (!t) return 0;
-    for (auto& op : t->net.ops) if (op.tc) tc_conv_free(op.tc);
-    for (void* p : t->net.owned) cudaFree(p);
     delete t;
     return 0;
 }
@@ -121,13 +77,7 @@ extern "C" int b200trk_tower_forward(b200trk_tower_t* t, const float* feat, cons
     const int n = (int)net->ops.size();
     for (int i = 0; i < n; ++i) {
         const Op& op = net->ops[i];
-        if (op.tc) {
-            if (int e = tc_conv_launch(net, op, S, st)) return e;
-        } else {
-            ConvShape sh{S, op.Hin, op.Win, op.Cin, op.Hout, op.Wout, op.Cout, op.k, op.stride, op.pad};
-            ConvEpilogue ep{op.bias, nullptr, 0};
-            if (int e = launch_conv_fp32(net->bufs[op.in], op.w, net->bufs[op.out], sh, ep, net->splitk_ws, net->splitk_ws_floats, net->sms, st)) return e;
-        }
+        if (int e = conv_step(net, op, S, st)) return e;
         if (stop()) return 0;
         if (i < n - 1) {
             groupnorm1_relu_kernel<<<S, 1024, 0, st>>>(net->bufs[op.out], t->gamma[i], t->beta[i], HW, op.Cout, 1e-5f);
@@ -143,8 +93,6 @@ extern "C" int b200trk_tower_forward(b200trk_tower_t* t, const float* feat, cons
 }
 
 // ---- debug read-back (tests): stop a forward pass after launch k, copy an activation buffer, report each convolution's launch plan ----
-namespace b200trk { int tc_conv_grid(const Op& op, int dims[4]); int tc_conv_reduction(const Op& op); int tc_conv_tile(const Op& op, int dims[2]); }
-
 extern "C" int b200trk_tower_debug_num_launches(const b200trk_tower_t* t) {
     return t ? 2 * (int)t->net.ops.size() + 1 : 0;
 }

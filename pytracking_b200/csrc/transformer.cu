@@ -11,21 +11,13 @@
 #include <cmath>
 #include <cstring>
 
-namespace b200trk {
-
-int tc_conv_prepare(b200trk_net* net, Op& op, const std::vector<float>& w_khwc);   // conv_tc.cu
-int tc_conv_launch(b200trk_net* net, const Op& op, int S, cudaStream_t st);
-void tc_conv_free(TcConv* tc);
-
-}  // namespace b200trk
-
 #include "transformer_kernels.cuh"      // add_pos, layernorm, small_linear, attention, attention_q1
 
 using namespace b200trk;
 
 struct b200trk_transformer {
     int D = 0, H = 0, FF = 0, L = 0, B = 0, n_enc = 0, n_dec = 0, M = 0;
-    b200trk_net box;                      // container for the GEMM plan: buffers, split-K workspace, SM count
+    b200trk_net box;                      // container for the GEMM plan and every device buffer: split-K workspace, SM count
     std::vector<Op> gemms;                // tensor-core GEMMs in execution order
     struct Lin { float *w = nullptr, *b = nullptr; };
     struct LN { float *g = nullptr, *b = nullptr; };
@@ -41,27 +33,6 @@ struct b200trk_transformer {
     int stop_after = -1;                  // debug: forward returns after this launch of its fixed sequence (-1: runs to the end)
 };
 
-static int t_alloc(b200trk_transformer* t, float** p, size_t floats) {
-    void* q = nullptr;
-    B200_CHECK_CUDA(cudaMalloc(&q, floats * sizeof(float)));
-    B200_CHECK_CUDA(cudaMemset(q, 0, floats * sizeof(float)));
-    t->box.owned.push_back(q);
-    *p = (float*)q;
-    return 0;
-}
-static int t_upload(b200trk_transformer* t, float** p, const float* host, size_t floats) {
-    if (int e = t_alloc(t, p, floats)) return e;
-    B200_CHECK_CUDA(cudaMemcpy(*p, host, floats * sizeof(float), cudaMemcpyHostToDevice));
-    return 0;
-}
-static int t_buf(b200trk_transformer* t, size_t floats, int* id) {
-    float* p = nullptr;
-    if (int e = t_alloc(t, &p, floats)) return e;
-    t->box.bufs.push_back(p);
-    t->box.buf_floats.push_back(floats);
-    *id = (int)t->box.bufs.size() - 1;
-    return 0;
-}
 // register y[M,N] = act(x[M,K] W^T + b) (+ res) as a 1x1 convolution over an (Ht x Wt) "image" of tokens
 static int t_gemm(b200trk_transformer* t, int in, int out, int res, const b200trk_transformer::Lin& lin, int K, int N, int relu, int* gid) {
     Op op;
@@ -71,17 +42,13 @@ static int t_gemm(b200trk_transformer* t, int in, int out, int res, const b200tr
     op.Win = op.Wout = Wt; op.Hin = op.Hout = t->M / Wt;
     op.Cin = K; op.Cout = N; op.k = 1; op.stride = 1; op.pad = 0; op.relu = relu;
     op.w = lin.w; op.bias = lin.b;
-    std::vector<float> unused;
-    if (int e = tc_conv_prepare(&t->box, op, unused)) return e;
+    if (int e = tc_conv_prepare(&t->box, op)) return e;
     t->gemms.push_back(op);
     *gid = (int)t->gemms.size() - 1;
     return 0;
 }
 
 extern "C" int b200trk_transformer_destroy(b200trk_transformer_t* t) {
-    if (!t) return 0;
-    for (auto& op : t->gemms) if (op.tc) tc_conv_free(op.tc);
-    for (void* p : t->box.owned) cudaFree(p);
     delete t;
     return 0;
 }
@@ -112,23 +79,23 @@ extern "C" int b200trk_transformer_create(b200trk_transformer_t** out, const b20
     const int D = d_model, M = t->M;
     int e = 0;
     t->box.splitk_ws_floats = (size_t)4 << 20;
-    if (!e) e = t_alloc(t, &t->box.splitk_ws, t->box.splitk_ws_floats);
-    if (!e) e = t_buf(t, (size_t)M * D, &t->b_src);
-    if (!e) e = t_buf(t, (size_t)M * D, &t->b_qkin);
-    if (!e) e = t_buf(t, (size_t)M * 2 * D, &t->b_qk);
-    if (!e) e = t_buf(t, (size_t)M * D, &t->b_v);
-    if (!e) e = t_buf(t, (size_t)M * D, &t->b_att);
-    if (!e) e = t_buf(t, (size_t)M * D, &t->b_tmp);
-    if (!e) e = t_buf(t, (size_t)M * dim_ff, &t->b_ff);
-    if (!e) e = t_buf(t, (size_t)M * D, &t->b_mem_pos);
-    if (!e) e = t_buf(t, (size_t)M * D, &t->b_k);
+    if (!e) e = t->box.mem.alloc(&t->box.splitk_ws, t->box.splitk_ws_floats, true);
+    if (!e) e = t->box.add_buf((size_t)M * D, &t->b_src, true);
+    if (!e) e = t->box.add_buf((size_t)M * D, &t->b_qkin, true);
+    if (!e) e = t->box.add_buf((size_t)M * 2 * D, &t->b_qk, true);
+    if (!e) e = t->box.add_buf((size_t)M * D, &t->b_v, true);
+    if (!e) e = t->box.add_buf((size_t)M * D, &t->b_att, true);
+    if (!e) e = t->box.add_buf((size_t)M * D, &t->b_tmp, true);
+    if (!e) e = t->box.add_buf((size_t)M * dim_ff, &t->b_ff, true);
+    if (!e) e = t->box.add_buf((size_t)M * D, &t->b_mem_pos, true);
+    if (!e) e = t->box.add_buf((size_t)M * D, &t->b_k, true);
     auto up_lin = [&](b200trk_transformer::Lin& l, const float* w, const float* b, size_t rows, size_t cols) {
-        if (!e) e = t_upload(t, &l.w, w, rows * cols);
-        if (!e && b) e = t_upload(t, &l.b, b, rows);
+        if (!e) e = t->box.mem.upload(&l.w, w, rows * cols);
+        if (!e && b) e = t->box.mem.upload(&l.b, b, rows);
     };
     auto up_ln = [&](b200trk_transformer::LN& n, const float* g, const float* b) {
-        if (!e) e = t_upload(t, &n.g, g, D);
-        if (!e) e = t_upload(t, &n.b, b, D);
+        if (!e) e = t->box.mem.upload(&n.g, g, D);
+        if (!e) e = t->box.mem.upload(&n.b, b, D);
     };
     t->enc.resize(n_enc);
     for (int i = 0; i < n_enc && !e; ++i) {
@@ -166,14 +133,14 @@ extern "C" int b200trk_transformer_create(b200trk_transformer_t** out, const b20
         if (!e) e = t_gemm(t, t->b_src, t->b_v, -1, Dl.ca_v, D, D, 0, &Dl.g_v);            // V = W_v memory
     }
     up_ln(t->dec_norm, dec_norm_w, dec_norm_b);
-    if (!e) e = t_alloc(t, &t->d_tgt, (size_t)B * D);
-    if (!e) e = t_alloc(t, &t->d_t1, (size_t)B * D);
-    if (!e) e = t_alloc(t, &t->d_t2, (size_t)B * D);
-    if (!e) e = t_alloc(t, &t->d_q, (size_t)B * D);
-    if (!e) e = t_alloc(t, &t->d_att, (size_t)B * D);
-    if (!e) e = t_alloc(t, &t->d_ff, (size_t)B * dim_ff);
-    if (!e) e = t_alloc(t, &t->d_qpos, (size_t)B * D);
-    if (e) { b200trk_transformer_destroy(t); return e; }
+    if (!e) e = t->box.mem.alloc(&t->d_tgt, (size_t)B * D, true);
+    if (!e) e = t->box.mem.alloc(&t->d_t1, (size_t)B * D, true);
+    if (!e) e = t->box.mem.alloc(&t->d_t2, (size_t)B * D, true);
+    if (!e) e = t->box.mem.alloc(&t->d_q, (size_t)B * D, true);
+    if (!e) e = t->box.mem.alloc(&t->d_att, (size_t)B * D, true);
+    if (!e) e = t->box.mem.alloc(&t->d_ff, (size_t)B * dim_ff, true);
+    if (!e) e = t->box.mem.alloc(&t->d_qpos, (size_t)B * D, true);
+    if (e) { delete t; return e; }
     *out = t;
     return 0;
 }
@@ -278,8 +245,6 @@ extern "C" int b200trk_transformer_forward(b200trk_transformer_t* t, const float
 }
 
 // ---- debug read-back (tests): stop a forward pass after launch k, copy any internal buffer, report each GEMM's launch plan ----
-namespace b200trk { int tc_conv_grid(const Op& op, int dims[4]); int tc_conv_reduction(const Op& op); int tc_conv_tile(const Op& op, int dims[2]); }
-
 extern "C" int b200trk_transformer_debug_num_launches(const b200trk_transformer_t* t) {
     return t ? 9 * t->n_enc + 1 + 13 * t->n_dec + 1 : 0;
 }
